@@ -1,11 +1,11 @@
 """Benchmark of the MAC-VO per-frame hot path (BASELINE.json metric: stereo frames/sec @640x480; corr-vol
 HBM GB/s vs roofline).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--config performant|fast]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--config performant|fast] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 One "step" = one stereo frame through the whole hot path: FlowFormerCov frontend (correlation volume +
-12 x window lookup on the sm_100a kernels, dense layers through cuDNN/cuBLAS, CUDA graph) -> fused dense
+12 x window lookup on the sm_90a kernels, dense layers through cuDNN/cuBLAS, CUDA graph) -> fused dense
 post-processing + keypoint scoring -> candidate selection -> device-side observation building (gathers, 2 x observation
 covariance, sanity filter, MatchObs packing) -> two-frame pose-graph LM solve -> mapping points, on a seeded synthetic TartanAir-shape 640x480 sequence with the
 MACVO_Performant settings (fp32 network, 200 keypoints, mapping on). `value` keeps the images resident in
@@ -15,6 +15,10 @@ optimised pose back every frame. N > 1 = N independent streams, one per GPU (BAS
 
 `--impl reference` times the reference's own CPU arithmetic (the oracle port, see oracle/) with all host
 threads on a bounded sample of the same workload.
+
+`--dump-outputs DIR` writes what the timed path returned for its last step (optimised pose, trajectory, packed
+observations and mapping points) as DIR/<name>.npy, float32 / float64; inputs are seeded, so two builds can be compared
+output for output.
 """
 from __future__ import annotations
 
@@ -114,7 +118,7 @@ def run_cpu(cfg: dict, frames_to_time: int, warm: int) -> dict:
     # 128 threads measured 178 s/frame on the GPU box against ~9 s/frame with 8; use what the path can use
     cores = min(os.cpu_count() or 1, int(os.environ.get("MACVO_BENCH_CPU_THREADS", 16)))
     torch.set_num_threads(cores)
-    # the B200 frontend (like the reference's CUDA-graph frontend) sets matmul precision "medium" process-wide; the
+    # the GPU frontend (like the reference's CUDA-graph frontend) sets matmul precision "medium" process-wide; the
     # reference's CPU path never does, and on CPUs with bf16 units "medium" changes fp32 matmuls -> pin "highest"
     prev_prec = torch.get_float32_matmul_precision()
     torch.set_float32_matmul_precision("highest")
@@ -171,7 +175,7 @@ def time_corr_kernel(device: str, iters: int = 10) -> dict:
         ops.corr_build(f1, f2)
     times = []
     for _ in range(iters):
-        flush.zero_()                                                      # evict L2 (126 MB) between launches
+        flush.zero_()                                                      # evict L2 (50 MB on H100) between launches
         s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         s.record()
         ops.corr_build(f1, f2)                                             # enqueued on torch's current stream
@@ -184,7 +188,33 @@ def time_corr_kernel(device: str, iters: int = 10) -> dict:
     return {"seconds": sum(times) / len(times), "bytes": algo_bytes, "mode": ops.CORR_MODE_NAMES[mode]}
 
 
-def run_gpu(cfg: dict, steps: int, warmup: int, n_gpus: int) -> dict:
+def dump_outputs(odo, out_dir: str) -> list[str]:
+    """The arrays a caller of the fused driver receives for the newest frame: its optimised pose, the trajectory so far and
+    the frame's packed observations / mapping points, one DIR/<name>.npy each (integers as float64). How many observations
+    and mapping points a frame has depends on the data, so those arrays are zero-padded to the driver's capacities
+    (num_point observations, num_map_point mapping points) and `obs_counts` says how many rows are valid: every file has
+    the same shape from build to build and none is empty."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    obs = odo.observations()
+    counts = [obs.pop(k) for k in ("num_obs", "num_kp", "num_selected", "status")]
+    n_map = 0
+    if "map_cov" in obs:
+        n_map = obs["map_cov"].shape[0]
+    arrays = {"pose": odo.latest_pose(), "trajectory": odo.finish(),
+              "obs_counts": torch.tensor(counts + [n_map], dtype=torch.float64)}
+    for k, v in obs.items():
+        rows = odo.num_map_point if k.startswith("map_") else odo.num_point
+        padded = torch.zeros((rows, *v.shape[1:]), dtype=v.dtype)
+        padded[:v.shape[0]] = v
+        arrays[f"obs_{k}"] = padded
+    for name, t in arrays.items():
+        a = t.detach().cpu()
+        np.save(os.path.join(out_dir, f"{name}.npy"), (a if a.dtype in (torch.float32, torch.float64) else a.double()).numpy())
+    return sorted(arrays)
+
+
+def run_gpu(cfg: dict, steps: int, warmup: int, n_gpus: int, dump_dir: str | None = None) -> dict:
     rank, world, local = _dist()
     assert torch.cuda.is_available(), "bench.py (GPU arm) needs CUDA; use --impl reference for the CPU arm"
     torch.cuda.set_device(local)
@@ -250,7 +280,8 @@ def run_gpu(cfg: dict, steps: int, warmup: int, n_gpus: int) -> dict:
         return ms, ops.LAUNCHES[0], odo
 
     with ClockSampler(local) as clk:
-        ms_dev, launches, _ = timed(frames_dev, read_pose=False)
+        ms_dev, launches, odo_dev = timed(frames_dev, read_pose=False)
+        dumped = dump_outputs(odo_dev, dump_dir) if dump_dir and rank == 0 else None
         ms_e2e, _, _ = timed(frames_host, read_pose=True)
         ms_api, _, _ = timed(frames_host, read_pose=True, fused=False)
     corr = time_corr_kernel(device)
@@ -259,14 +290,14 @@ def run_gpu(cfg: dict, steps: int, warmup: int, n_gpus: int) -> dict:
     if os.path.exists(peaks_path):
         peak, peak_src = json.load(open(peaks_path))["hbm_gbs"], "MEASURED_PEAKS.json hbm_gbs (measured copy bandwidth)"
     else:
-        peak, peak_src = 6650.0, "fallback of B200_PROFILING.md (MEASURED_PEAKS.json absent)"
+        peak, peak_src = 3350.0, "H100 SXM data-sheet HBM3 bandwidth, not measured (MEASURED_PEAKS.json absent)"
     traffic, traffic_src = None, None
     tpath = os.path.join(REPO, "profiles", "corr_tc_traffic.json")
     if os.path.exists(tpath):       # NOT measured in this run: dram__bytes_read.sum + dram__bytes_write.sum of one `ncu --set full` capture
         tj = json.load(open(tpath))
         traffic = tj.get(corr["mode"], tj).get("dram_bytes_per_launch")
         traffic_src = tj.get(corr["mode"], tj).get("source")
-    kernel_names = {"tf32": "macvo_corr_build: corr_tc_kernel<2> (tcgen05 kind::tf32, one pass over the fp32 K-major features, no pre-pass)",
+    kernel_names = {"tf32": "macvo_corr_build: corr_tc_kernel<2> (wgmma tf32, one pass over the fp32 K-major features, no pre-pass)",
                     "tc3": "macvo_corr_build: fp16 hi/lo operand split + corr_tc_kernel<3>",
                     "tc1": "macvo_corr_build: fp16 operand rounding + corr_tc_kernel<1>", "simt": "corr_simt_kernel"}
     achieved = corr["bytes"] / corr["seconds"] / 1e9
@@ -277,11 +308,11 @@ def run_gpu(cfg: dict, steps: int, warmup: int, n_gpus: int) -> dict:
         "data": "synthetic (seeded smoothed-noise TartanAir-shape stereo sequence, synthetic:0 network weights)",
         "config": {"workload": workload_name(cfg),
                    "streams": world, "parallelism": "replicas only (one independent stream per GPU, no collective)",
-                   "l2": "per-frame working set (184 MB correlation volume + >1 GB activations) exceeds the 126 MB L2; "
+                   "l2": "per-frame working set (184 MB correlation volume + >1 GB activations) exceeds the 50 MB L2; "
                          "the corr roofline loop flushes L2 with a 256 MB write between launches",
                    "matmul_precision": "TF32 like the reference GPU frontend (Frontend.py:275-277): cuDNN / cuBLAS layers, our attention / "
-                                       "PatchEmbed kernels and the correlation volume (kind::tf32); the decoder's SepConvGRU units and 3x3 / 1x1 "
-                                       "convolutions on our tcgen05 kernels with fp16 operands (11-bit significand), fp32 accumulation "
+                                       "PatchEmbed kernels and the correlation volume (wgmma tf32); the decoder's SepConvGRU units and 3x3 / 1x1 "
+                                       "convolutions on our wgmma kernels with fp16 operands (11-bit significand), fp32 accumulation "
                                        "and fp32 recurrent state; token path, LayerNorm, lookup, "
                                        "post-processing, covariance fp32; LM fp64. Parity of this mode at this shape: "
                                        "tests/test_gpu_parity_ladder.py (flow 9e-4 of its scale vs float64 truth; strict-fp32 mode 2.5e-6)"},
@@ -302,6 +333,8 @@ def run_gpu(cfg: dict, steps: int, warmup: int, n_gpus: int) -> dict:
                      "peak_source": peak_src, "algorithmic_bytes_per_launch": corr["bytes"],
                      "launch_seconds": corr["seconds"]},
     }
+    if dumped is not None:
+        out["dumped_outputs"] = {"dir": dump_dir, "arrays": dumped}
     if rank == 0 and world == 1:
         out["cpu_baseline"] = run_cpu(cfg, frames_to_time=1, warm=0)
     if world > 1:
@@ -419,6 +452,8 @@ def main() -> None:
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--config", default="performant", choices=list(CONFIGS) + ["sharded"])
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the timed path's outputs of its last step as DIR/<name>.npy (GPU arm, 640x480 configs)")
     a = ap.parse_args()
     a.warmup = max(a.warmup, 3) if a.impl == "b200" else a.warmup
     rank, world, _ = _dist()
@@ -443,7 +478,7 @@ def main() -> None:
                 "cpu_baseline": r, "e2e": {"value": r["value"], "unit": "frames/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0}}
         print(json.dumps(line), flush=True)
         return
-    out = run_gpu(cfg, a.steps, a.warmup, a.gpus)
+    out = run_gpu(cfg, a.steps, a.warmup, a.gpus, a.dump_outputs)
     if rank == 0:
         print(json.dumps(out), flush=True)
 

@@ -1,5 +1,5 @@
 /*
- * macvo_b200.h — C ABI of the B200 (sm_100a) hot path for MAC-VO.
+ * macvo_b200.h — C ABI of the H100 (sm_90a) hot path for MAC-VO.
  *
  * MAC-VO's plugin boundary is a Python class registry (SURVEY.md §8b), not an FFI; this header is
  * the thin C layer BELOW the plugin classes (`mac-vo_b200/plugins.py`). Every entry point takes raw
@@ -27,7 +27,7 @@ extern "C" {
 #define MACVO_E_UNSUPPORTED (-3)/* mode not available for these shapes on this device              */
 #define MACVO_E_DRIVER (-4)     /* driver entry point (cuTensorMapEncodeTiled) could not be loaded */
 
-/* library identification: "macvo_b200 <version> sm_100a" */
+/* library identification: "macvo_b200 <version> sm_90a" */
 const char* macvo_b200_version(void);
 
 /* ------------------------------------------------------------------------------------------------
@@ -41,17 +41,17 @@ const char* macvo_b200_version(void);
  * (B, 1, H1, W1, H1, W1) tensor the cost perceiver and the decoder view.
  *
  * mode: MACVO_CORR_SIMT      fp32 FFMA shared-memory tiled kernel (reference-accuracy baseline)
- *       MACVO_CORR_TC_3XF16  tcgen05 (5th-gen tensor core) kernel: each fp32 operand is split into
- *                            fp16 hi + lo; hi*hi + hi*lo + lo*hi accumulated in fp32 TMEM
+ *       MACVO_CORR_TC_3XF16  wgmma (tensor core) kernel: each fp32 operand is split into
+ *                            fp16 hi + lo; hi*hi + hi*lo + lo*hi accumulated in fp32
  *                            (~2^-22 relative product error: fp32-class accuracy)
- *       MACVO_CORR_TC_1XF16  tcgen05, operands rounded to fp16 once (MACVO_Fast: fp16 encoder)
+ *       MACVO_CORR_TC_1XF16  wgmma, operands rounded to fp16 once (MACVO_Fast: fp16 encoder)
  * The tensor-core modes need dim % 64 == 0 and n % 8 == 0 and a workspace of
  * macvo_corr_workspace_bytes() bytes (device memory, 1024-byte aligned).
  */
 #define MACVO_CORR_SIMT 0
 #define MACVO_CORR_TC_3XF16 1
 #define MACVO_CORR_TC_1XF16 2
-#define MACVO_CORR_TC_TF32 3   /* tcgen05 kind::tf32, ONE pass straight over the fp32 K-major (channels_last) features: no
+#define MACVO_CORR_TC_TF32 3   /* wgmma tf32, ONE pass straight over the fp32 K-major (channels_last) features: no
                                 * operand pre-pass, no workspace; operands truncated to TF32 by the tensor core (10-bit
                                 * mantissa) = what the reference's own torch.matmul does for this product once its frontend
                                 * has set allow_tf32 (Frontend.py:275-277). Requires MACVO_CORR_KMAJOR_INPUT. */
@@ -322,7 +322,7 @@ int macvo_gru_gates(const float* zr, const float* bias, const float* hx, float* 
 /* hx[:, :128] <- (1 - z) * hx[:, :128] + z * tanh(q + bias); bias (128) may be NULL; optional dense copy (pixels,128) */
 int macvo_gru_blend(const float* q, const float* bias, const float* z, float* hx, float* h_dense, long long pixels,
                     void* stream);
-/* ---- decoder convolutions on tcgen05 (csrc/conv_tc.cu): 3x3 (padding 1) / 1x1 convolutions of the motion encoder, the GMA value
+/* ---- decoder convolutions on wgmma (csrc/conv_tc.cu): 3x3 (padding 1) / 1x1 convolutions of the motion encoder, the GMA value
  * projection, the flow head and the covariance head (core/gru.py:6-14,45-64, gma.py:84-130, FlowFormerCov/covhead.py:20-58) as
  * implicit GEMMs over fp16 pixel rows in "layout U" (csrc/rows_layout.cuh): image b, pixel (y, x) lives at row
  * 2 + (b (H + 4) + y + 2)(W + 4) + x + 2 of a zero-initialised buffer of macvo_rows_count(batch, H, W, 0) rows; the kernels only
@@ -350,7 +350,7 @@ int macvo_conv_tc(const void* in_rows, int in_channels, int in_dense, const void
 int macvo_flow_im2col(const float* coords1, const float* coords0, void* rows, float* mf32, void* mf16_rows, int batch,
                       int height, int width, void* stream);
 
-/* ---- SepConvGRU on tcgen05 (csrc/gru_conv_tc.cu): the 1x5 / 5x1 gate convolutions of gru.py:22-43 as implicit GEMMs with the
+/* ---- SepConvGRU on wgmma (csrc/gru_conv_tc.cu): the 1x5 / 5x1 gate convolutions of gru.py:22-43 as implicit GEMMs with the
  * gate math in the epilogue, for `units` (1 or 2: flow, covariance — covhead.py:95-131) recurrent units per launch.
  * Operands are fp16 PADDED pixel rows: pass `vertical` = 0 (1x5) uses layout U (above), `vertical` = 1 (5x1) stores pixel
  * (b, y, x) at row 2 + (b W + x)(H + 4) + y + 2; all other rows must be zero (allocate

@@ -1,4 +1,4 @@
-"""mac-vo_b200: B200-native (sm_100a) hot path for MAC-VO behind its Module plugin interfaces.
+"""mac-vo_b200: H100-native (sm_90a) hot path for MAC-VO behind its Module plugin interfaces.
 
 Import as `macvo_b200` (alias package at the repo root). See DESIGN.md / INTEGRATION.md.
 """

@@ -1,4 +1,4 @@
-"""Build recipe: compile csrc/*.cu for sm_100a into ONE in-tree shared library with a C ABI.
+"""Build recipe: compile csrc/*.cu for sm_90a (H100) into ONE in-tree shared library with a C ABI.
 
     python -m macvo_b200.build        (or  __graft_entry__.build())
 
@@ -20,7 +20,7 @@ LIB_PATH = os.path.join(LIB_DIR, "libmacvo_b200.so")
 SOURCES = ["corr_build.cu", "corr_build_simt.cu", "corr_build_tc.cu", "corr_lookup.cu", "dense_select.cu",
            "cov2to3.cu", "pgo.cu", "nn_kernels.cu", "decoder_fused.cu", "observe.cu", "decoder_token.cu", "motion_interp.cu",
            "gru_conv_tc.cu", "conv_tc.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "--use_fast_math=false"]
 
 
@@ -62,7 +62,7 @@ def build(force: bool = False, verbose: bool = True) -> str:
             raise RuntimeError(f"nvcc failed on {src}:\n{out}")
         if verbose and out.strip():
             print(out, file=sys.stderr)
-    link = [nvcc, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", LIB_PATH, *objs, "-lcuda" if False else "-lcudart_static",
+    link = [nvcc, "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", LIB_PATH, *objs, "-lcuda" if False else "-lcudart_static",
             "-Xlinker", "--no-undefined", "-lpthread", "-ldl", "-lrt"]
     r = subprocess.run(link, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     if r.returncode != 0:

@@ -1,66 +1,57 @@
 // (f2) The decoder's 3x3 / 1x1 convolutions (motion encoder, GMA value projection, flow head, covariance head:
-// Module/Network/FlowFormer/core/gru.py:45-64,6-14, gma.py:84-130, FlowFormerCov/covhead.py:20-58) as tcgen05 implicit GEMMs.
+// Module/Network/FlowFormer/core/gru.py:45-64,6-14, gma.py:84-130, FlowFormerCov/covhead.py:20-58) as wgmma implicit GEMMs.
 //
 //   out[pixel, n] = act( bias[n] + sum_{tap, c} in[pixel + offset(tap), c] * w[n, tap, c] )
 //
-// rows = pixels, fp16 operands (11-bit significand >= TF32's 10), fp32 accumulation in TMEM. Activations live in layout U
+// rows = pixels, fp16 operands (11-bit significand >= TF32's 10), fp32 accumulation in registers. Activations live in layout U
 // (csrc/rows_layout.cuh: one fp16 row per pixel, 2 zero pixels around every image), so a 3x3 tap is a row offset and a
-// tile is any 128 consecutive rows. Per 64-channel block and per tap ROW dy one A tile of 136 rows is loaded by TMA and
-// reused by the three dx taps through the UMMA descriptor start (+128 B per pixel; the 128-byte swizzle is address based —
-// profiles/r02_umma_descriptor_shift_probe.log). A 1x1 convolution may also read plain dense pixel rows.
+// tile is any 128 consecutive rows: per 64-channel block and tap, TMA loads the 128 shifted input rows and the tap's filter
+// rows into one ring slot (rows outside the buffer are zero filled). A 1x1 convolution may also read plain dense pixel rows.
 //
-// One CTA PAIR (cta_group::2, M = 256) per (two 128-pixel tiles, slice of output channels): each CTA stages its own A tile and
-// HALF of the filter rows of every step (a first single-CTA version ran at 1/4 of its MMA bound: 10 KB of shared-memory
-// operand reads per 96-cycle MMA on top of the TMA fill traffic); warp 0 = TMA producer, warp 1 = MMA issuer (leader), warps 2..9 = epilogue
-// (TMEM -> registers -> XOR-swizzled smem transpose in the idle operand ring -> bias / ReLU -> row-contiguous global stores
-// as fp16 rows for the next convolution and / or fp32 dense rows). Launched with programmatic stream serialization: the
-// weights of the first ring slots are in flight before `griddepcontrol.wait` lets the input rows be touched.
+// One CTA per (128-pixel tile, slice of N output channels): warps 0..7 = two consumer warpgroups (m64nNk16 wgmma, one
+// MMA group kept in flight), warp 8 = TMA producer. Epilogue: accumulators -> XOR-swizzled smem transpose in the idle
+// operand ring -> bias / ReLU -> row-contiguous global stores as fp16 rows for the next convolution and / or fp32 dense rows.
+// Launched with programmatic stream serialization: the filters of the first ring slots are in flight before
+// `griddepcontrol.wait` lets the input rows be touched.
 #include "tc_common.cuh"
 #include "rows_layout.cuh"
 #include <cuda_fp16.h>
 
 namespace {
 
-constexpr int TILE_M = macvo_rows::TILE_M, BLOCK_K = 64, UMMA_K = 16;
-constexpr int A_ROWS = 136, A_BYTES = A_ROWS * 128;
-constexpr int EPI_WARPS = 8, THREADS = 32 * (2 + EPI_WARPS);
+constexpr int TILE_M = macvo_rows::TILE_M, BLOCK_K = 64;
+constexpr int A_BYTES = TILE_M * 128;                          // 16 KB: 128 rows x 64 fp16
 constexpr int SMEM_MAX = 200 * 1024;
 
 struct ConvArgs {
     int taps, kblocks;            // 1 | 9 ; input channels / 64
-    int n_cta;                    // output channels per CTA pair = UMMA N (multiple of 32, <= 256); grid.y slices
-    int tmem_cols, slots;         // TMEM columns (power of two >= n_cta), ring depth in groups
+    int slots;                    // ring depth
     int in_dense;                 // A rows are dense pixel rows (1x1 only) instead of layout U
     int batch, height, width, wp; // wp = width + 4
     int m_rows;                   // rows to cover: pixels (dense) or padded pixels (layout U)
     int relu, n_valid;            // columns >= n_valid are computed (zero filters) but never stored
-    const float* bias;            // (grid.y * n_cta) or NULL
+    const float* bias;            // (grid.y * N) or NULL
     __half* out16; int out16_pitch, out16_off, out16_dense;
     float* out32; int out32_pitch, out32_off;
     int out32_planes;             // 1: out32 is a (batch, n_valid, H, W) map and the result is ADDED to it (coords += delta)
-    uint32_t idesc;
     Timeline tl;                  // profiling aid, buf == NULL in production
     unsigned long long* trace;    // profiling aid: [role][64] globaltimer events of block (0, 0)
 };
 
-__global__ void __launch_bounds__(THREADS, 1)
+// N = output channels per CTA (multiple of 32, <= 256); grid.y slices the padded output channels
+template <int N>
+__global__ void __launch_bounds__(TC_THREADS, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_w, ConvArgs a) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    // ring of `slots` group slots: [A tile 17 KB | this CTA's half of the filter rows of the group's 1 or 3 taps]
-    const int tpg = a.taps == 9 ? 3 : 1;                       // taps served by one A tile = taps per group
-    const int b_bytes = (a.n_cta / 2) * 128;
-    const int slot_bytes = A_BYTES + tpg * b_bytes;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + a.slots * slot_bytes);
-    const uint32_t bar_full = smem_u32(bars), bar_empty = bar_full + 8 * a.slots, bar_tfull = bar_empty + 8 * a.slots;
-    uint32_t* tmem_base_slot = reinterpret_cast<uint32_t*>(bars + 2 * a.slots + 1);
+    // ring of `slots` slots: [A tile 16 KB | the tap's N filter rows]
+    constexpr int SLOT_BYTES = A_BYTES + N * 128;
+    const uint32_t bar_full = smem_u32(smem + a.slots * SLOT_BYTES), bar_empty = bar_full + 8 * a.slots;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t rank = cluster_ctarank();
-    const bool leader = rank == 0;
-    const int tile = (int)(blockIdx.x & ~1u) + (int)rank, slice = blockIdx.y;
+    const int tile = blockIdx.x, slice = blockIdx.y;
     Timeline tl = a.tl;
-    tl.begin(100 + a.taps * 1000 + a.kblocks * 10000 + a.n_cta * 100000);
+    tl.begin(100 + a.taps * 1000 + a.kblocks * 10000 + N * 100000);
     int tr_n = 0;
     auto TR = [&](int role) {
         if (a.trace != nullptr && blockIdx.x == 0 && blockIdx.y == 0 && tr_n < 64) {
@@ -69,180 +60,146 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
             a.trace[role * 64 + tr_n++] = t;
         }
     };
-    if (warp == 2 && lane == 0) TR(2);
-    const int ngroups = a.kblocks * (a.taps == 9 ? 3 : 1);
+    if (warp == 0 && lane == 0) TR(2);
+    const int steps = a.kblocks * a.taps;
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < a.slots; ++s) { mbar_init(bar_full + 8 * s, 1); mbar_init(bar_empty + 8 * s, 1); }
-        mbar_init(bar_tfull, 1);
+        for (int s = 0; s < a.slots; ++s) { mbar_init(bar_full + 8 * s, 1); mbar_init(bar_empty + 8 * s, 2); }
         fence_barrier_init();
         prefetch_tmap(&map_a); prefetch_tmap(&map_w);
     }
-    if (warp == 1) tmem_alloc(smem_u32(tmem_base_slot), a.tmem_cols);
-    tc_fence_before();
     __syncthreads();
-    cluster_sync_all();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_base_slot;
     asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
 
-    if (warp == 0) {
-        // ===================== TMA producer (both CTAs; completion lands on the leader's barriers) =====================
-        // One request per operand and GROUP (a tap row of a 64-channel block): the filter box is the 3-D view (64 channels, rows,
-        // dx) of the (n, tap, c) matrix, so the three dx taps arrive as three consecutive swizzled tiles. All indices are running
-        // counters: a first version issued one request per tap and derived its indices with `/` and `%` by run-time values —
-        // those integer divisions, not the loads or the MMAs, set its pace (0.41 us per step for every N).
+    if (warp == TC_PRODUCER_WARP) {
+        // ===================== TMA producer =====================
+        // steps run over (64-channel block, tap), taps fastest; all indices are running counters
         if (elect_one()) {
             const int c_in = a.kblocks * BLOCK_K;
-            const int brow = slice * a.n_cta + (int)rank * (a.n_cta / 2);
             const int base_row = a.in_dense ? tile * TILE_M : macvo_rows::GUARD + tile * TILE_M;
-            int slot = 0, kb = 0, dy = a.taps == 9 ? 0 : 1;
-            uint32_t phase = 0;
-            auto issue_b = [&](int sl, int kb_, int dy_) {                  // filters of one group -> slot sl (after the A tile)
+            auto issue_w = [&](int sl, int kb_, int tap_) {                 // filters of one step -> slot sl (after the A tile)
                 const uint32_t full = bar_full + 8 * sl;
-                if (leader) mbar_expect_tx(full, 2 * slot_bytes);          // A + filters, from both CTAs
-                tma_load_3d_2cta(smem_u32(smem + sl * slot_bytes + A_BYTES), &map_w, full,
-                                 (a.taps == 9 ? dy_ * 3 * c_in : 0) + kb_ * BLOCK_K, brow, 0);
+                mbar_expect_tx(full, SLOT_BYTES);                          // A + filters
+                tma_load_2d(smem_u32(smem + sl * SLOT_BYTES + A_BYTES), &map_w, full, tap_ * c_in + kb_ * BLOCK_K, slice * N);
             };
-            auto issue_a = [&](int sl, int kb_, int dy_) {
-                tma_load_2d_2cta(smem_u32(smem + sl * slot_bytes), &map_a, bar_full + 8 * sl, kb_ * BLOCK_K,
-                                 base_row + (a.taps == 9 ? (dy_ - 1) * a.wp - 1 : 0));
+            auto issue_a = [&](int sl, int kb_, int tap_) {                 // tap (dy, dx) = row offset (dy - 1) wp + dx - 1
+                const int off = a.taps == 9 ? (tap_ / 3 - 1) * a.wp + tap_ % 3 - 1 : 0;
+                tma_load_2d(smem_u32(smem + sl * SLOT_BYTES), &map_a, bar_full + 8 * sl, kb_ * BLOCK_K, base_row + off);
             };
-            auto advance = [&](int& kb_, int& dy_) { if (a.taps == 9) { if (++dy_ == 3) { dy_ = 0; ++kb_; } } else ++kb_; };
-            // the filters of the first `slots` groups do not depend on the previous kernel: in flight before the wait
-            const int pre = ngroups < a.slots ? ngroups : a.slots;
-            { int k2 = kb, d2 = dy; for (int g = 0; g < pre; ++g) { issue_b(g, k2, d2); advance(k2, d2); } }
+            auto advance = [&](int& kb_, int& tap_) { if (++tap_ == a.taps) { tap_ = 0; ++kb_; } };
+            // the filters of the first `slots` steps do not depend on the previous kernel: in flight before the wait
+            const int pre = steps < a.slots ? steps : a.slots;
+            { int k2 = 0, t2 = 0; for (int g = 0; g < pre; ++g) { issue_w(g, k2, t2); advance(k2, t2); } }
             asm volatile("griddepcontrol.wait;" ::: "memory");
             TR(0);
-            for (int g = 0; g < ngroups; ++g) {
+            int slot = 0, kb = 0, tap = 0;
+            uint32_t phase = 0;
+            for (int g = 0; g < steps; ++g) {
                 if (g >= pre) {
                     mbar_wait(bar_empty + 8 * slot, phase ^ 1);
-                    issue_b(slot, kb, dy);
+                    issue_w(slot, kb, tap);
                 }
-                issue_a(slot, kb, dy);
+                issue_a(slot, kb, tap);
                 TR(0);
-                advance(kb, dy);
+                advance(kb, tap);
                 if (++slot == a.slots) { slot = 0; phase ^= 1; }
             }
         }
-    } else if (warp == 1) {
-        // ===================== MMA issuer: leader CTA, cta_group::2 =====================
-        if (leader) {
-            int slot = 0; uint32_t phase = 0;
-            for (int g = 0; g < ngroups; ++g) {
-                mbar_wait(bar_full + 8 * slot, phase);
-                tc_fence_after();
-                if (lane == 0) TR(1);
-                if (elect_one()) {
-                    const uint32_t sa = smem_u32(smem + slot * slot_bytes);
-                    for (int j = 0; j < tpg; ++j) {
-                        const uint64_t da = make_kmajor_sw128_desc(sa + j * 128);                   // dx tap = one pixel row further
-                        const uint64_t db = make_kmajor_sw128_desc(sa + A_BYTES + j * b_bytes);
-#pragma unroll
-                        for (int k = 0; k < BLOCK_K / UMMA_K; ++k)
-                            umma_f16_ss2(tmem_base, da + 2 * k, db + 2 * k, a.idesc, (g | j | k) != 0);
-                    }
-                    umma_commit_mc(bar_empty + 8 * slot, 3);
-                    if (g == ngroups - 1) umma_commit_mc(bar_tfull, 3);
-                }
-                __syncwarp();
-                if (++slot == a.slots) { slot = 0; phase ^= 1; }
-            }
-        }
-    } else {
-        // ===================== epilogue =====================
-        const int quarter = warp & 3, half = (warp - 2) >> 2;
-        const int m = quarter * 32 + lane;
-        const int r_in = tile * TILE_M + m;                       // dense pixel | padded pixel of this accumulator row
-        bool valid = r_in < a.m_rows;
-        int dense = 0, urow = 0;
-        if (valid) {
-            int b, y, x;
-            if (a.in_dense) {
-                x = r_in % a.width; y = (r_in / a.width) % a.height; b = r_in / (a.width * a.height);
-            } else {
-                const int line = r_in / a.wp;
-                x = r_in - line * a.wp - 2;
-                b = line / (a.height + 4);
-                y = line - b * (a.height + 4) - 2;
-                valid = x >= 0 && x < a.width && y >= 0 && y < a.height;
-            }
-            if (valid) {
-                dense = (b * a.height + y) * a.width + x;
-                urow = (int)macvo_rows::urow(b, y, x, a.height, a.width);
-            }
-        }
-        const uint32_t vmask = __ballot_sync(0xffffffffu, valid);
-        const int pitch = a.n_cta * 4;                            // staging row pitch (bytes), a multiple of 128
-        const uint32_t stage_q = smem_u32(smem) + quarter * 32 * pitch;
-        asm volatile("griddepcontrol.wait;" ::: "memory");        // nothing of the previous kernel is overwritten before it finished
-        if (warp == 2 && lane == 0) TR(2);
-        mbar_wait(bar_tfull, 0);
-        tc_fence_after();
-        if (warp == 2 && lane == 0) TR(2);
-        const uint32_t trow = tmem_base + ((uint32_t)(quarter * 32) << 16);
-        const int chunks = a.n_cta / 32, c_mid = (chunks + 1) / 2;
-        {
-            uint32_t r[32];
-            for (int c = half ? c_mid : 0; c < (half ? chunks : c_mid); ++c) {
-                tmem_ld_32x32b_x32(trow + c * 32, r);
-                tmem_ld_wait();
-#pragma unroll
-                for (int e = 0; e < 8; ++e)
-                    sts128(stage_q + lane * pitch + (((c * 8 + e) ^ (lane & 7)) << 4),
-                           make_float4(__uint_as_float(r[4 * e]), __uint_as_float(r[4 * e + 1]), __uint_as_float(r[4 * e + 2]),
-                                       __uint_as_float(r[4 * e + 3])));
-            }
-        }
-        asm volatile("bar.sync %0, 64;" ::"r"(1 + quarter) : "memory");      // both warps of the quarter staged their columns
-        // warp `half` finishes rows [16 half, +16) of the quarter: one full row per instruction, 4 columns per lane
-        // (every lane runs every iteration — the shuffles below need the whole warp; lanes past the slice only skip the stores)
-        for (int cg = 0; cg * 128 < a.n_cta; ++cg) {
-            const int col = cg * 128 + 4 * lane, gcol = slice * a.n_cta + col;
-            const bool lane_on = col < a.n_cta;
-            float4 bb = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (a.bias && lane_on) bb = __ldg(reinterpret_cast<const float4*>(a.bias + gcol));
-            const int nv = lane_on ? a.n_valid - gcol : 0;       // valid columns among this lane's 4
-#pragma unroll 4
-            for (int i = 0; i < 16; ++i) {
-                const int rr = half * 16 + i;
-                const long long d = __shfl_sync(0xffffffffu, dense, rr), ur = __shfl_sync(0xffffffffu, urow, rr);
-                if (!((vmask >> rr) & 1u) || nv <= 0) continue;
-                float4 v = lds128(stage_q + rr * pitch + (((col >> 2) ^ (rr & 7)) << 4));
-                v.x += bb.x; v.y += bb.y; v.z += bb.z; v.w += bb.w;
-                if (a.relu) { v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); v.z = fmaxf(v.z, 0.f); v.w = fmaxf(v.w, 0.f); }
-                if (a.out32 && a.out32_planes) {
-                    const long long hw = (long long)a.height * a.width, img = d / hw;
-                    float* o = a.out32 + (img * a.n_valid + gcol) * hw + (d - img * hw);
-                    o[0] += v.x; if (nv > 1) o[hw] += v.y; if (nv > 2) o[2 * hw] += v.z; if (nv > 3) o[3 * hw] += v.w;
-                } else if (a.out32) {
-                    float* o = a.out32 + d * a.out32_pitch + a.out32_off + gcol;
-                    if (nv >= 4 && ((a.out32_pitch | a.out32_off) & 3) == 0) *reinterpret_cast<float4*>(o) = v;
-                    else { o[0] = v.x; if (nv > 1) o[1] = v.y; if (nv > 2) o[2] = v.z; if (nv > 3) o[3] = v.w; }
-                }
-                if (a.out16) {
-                    // saturate instead of overflowing to inf (activations here are O(10); this is a guard, not a code path)
-                    const float lim = 65504.f;
-                    __half2 h2[2] = {__floats2half2_rn(fminf(fmaxf(v.x, -lim), lim), fminf(fmaxf(v.y, -lim), lim)),
-                                     __floats2half2_rn(fminf(fmaxf(v.z, -lim), lim), fminf(fmaxf(v.w, -lim), lim))};
-                    __half* o = a.out16 + (a.out16_dense ? d : ur) * a.out16_pitch + a.out16_off + gcol;
-                    if (nv >= 4) *reinterpret_cast<uint2*>(o) = *reinterpret_cast<uint2*>(h2);
-                    else { o[0] = __low2half(h2[0]); if (nv > 1) o[1] = __high2half(h2[0]); if (nv > 2) o[2] = __low2half(h2[1]); }
-                }
-            }
-        }
+        return;
     }
 
-    if (warp == 2 && lane == 0) TR(2);
-    tc_fence_before();
-    __syncthreads();
-    cluster_sync_relaxed();                   // no CTA exits while its peer may still signal / read its shared memory
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, a.tmem_cols);
+    // ===================== consumers: MMAs =====================
+    const int wg = warp >> 2;
+    float acc[N / 2];
+    {
+        int slot = 0, prev = 0; uint32_t phase = 0;
+        for (int g = 0; g < steps; ++g) {
+            mbar_wait(bar_full + 8 * slot, phase);
+            if (warp == 0 && lane == 0) TR(1);
+            const uint32_t sa = smem_u32(smem + slot * SLOT_BYTES);
+            const uint64_t da = make_kmajor_sw128_desc(sa + wg * 64 * 128), db = make_kmajor_sw128_desc(sa + A_BYTES);
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < BLOCK_K / 16; ++k) Wgmma<N>::f16(acc, da + 2 * k, db + 2 * k, (g | k) != 0);
+            wgmma_commit();
+            wgmma_wait<1>();                                       // the previous step's MMAs retired: release its slot
+            if (g > 0 && (threadIdx.x & 127) == 0) mbar_arrive(bar_empty + 8 * prev);
+            prev = slot;
+            if (++slot == a.slots) { slot = 0; phase ^= 1; }
+        }
+        wgmma_wait<0>();
+        fence_acc(acc);
     }
-    tl.end();
-    if (warp == 2 && lane == 0) TR(2);
+
+    // ===================== epilogue =====================
+    // rows of 4 N bytes, 16-byte chunks XOR-swizzled by the row: conflict-free both ways; warp (quarter, half) then finishes
+    // rows [32 quarter + 16 half, +16): one full row per instruction, 4 columns per lane
+    const int pitch = N * 4;
+    consumers_sync();                                              // every MMA of both warpgroups read its operands
+    stage_acc_rows<N>(smem_u32(smem) + wg * 64 * pitch, pitch, acc, 0);
+    const int quarter = warp & 3, half = warp >> 2;
+    const int m = quarter * 32 + lane;
+    const int r_in = tile * TILE_M + m;                           // dense pixel | padded pixel of this accumulator row
+    bool valid = r_in < a.m_rows;
+    int dense = 0, urow = 0;
+    if (valid) {
+        int b, y, x;
+        if (a.in_dense) {
+            x = r_in % a.width; y = (r_in / a.width) % a.height; b = r_in / (a.width * a.height);
+        } else {
+            const int line = r_in / a.wp;
+            x = r_in - line * a.wp - 2;
+            b = line / (a.height + 4);
+            y = line - b * (a.height + 4) - 2;
+            valid = x >= 0 && x < a.width && y >= 0 && y < a.height;
+        }
+        if (valid) {
+            dense = (b * a.height + y) * a.width + x;
+            urow = (int)macvo_rows::urow(b, y, x, a.height, a.width);
+        }
+    }
+    const uint32_t vmask = __ballot_sync(0xffffffffu, valid);
+    const uint32_t stage_q = smem_u32(smem) + quarter * 32 * pitch;
+    asm volatile("griddepcontrol.wait;" ::: "memory");            // nothing of the previous kernel is overwritten before it finished
+    consumers_sync();                                              // all rows staged
+    if (warp == 0 && lane == 0) TR(2);
+    // (every lane runs every iteration — the shuffles below need the whole warp; lanes past the slice only skip the stores)
+    for (int cg = 0; cg * 128 < N; ++cg) {
+        const int col = cg * 128 + 4 * lane, gcol = slice * N + col;
+        const bool lane_on = col < N;
+        float4 bb = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (a.bias && lane_on) bb = __ldg(reinterpret_cast<const float4*>(a.bias + gcol));
+        const int nv = lane_on ? a.n_valid - gcol : 0;       // valid columns among this lane's 4
+#pragma unroll 4
+        for (int i = 0; i < 16; ++i) {
+            const int rr = half * 16 + i;
+            const long long d = __shfl_sync(0xffffffffu, dense, rr), ur = __shfl_sync(0xffffffffu, urow, rr);
+            if (!((vmask >> rr) & 1u) || nv <= 0) continue;
+            float4 v = lds128(stage_q + rr * pitch + (((col >> 2) ^ (rr & 7)) << 4));
+            v.x += bb.x; v.y += bb.y; v.z += bb.z; v.w += bb.w;
+            if (a.relu) { v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); v.z = fmaxf(v.z, 0.f); v.w = fmaxf(v.w, 0.f); }
+            if (a.out32 && a.out32_planes) {
+                const long long hw = (long long)a.height * a.width, img = d / hw;
+                float* o = a.out32 + (img * a.n_valid + gcol) * hw + (d - img * hw);
+                o[0] += v.x; if (nv > 1) o[hw] += v.y; if (nv > 2) o[2 * hw] += v.z; if (nv > 3) o[3 * hw] += v.w;
+            } else if (a.out32) {
+                float* o = a.out32 + d * a.out32_pitch + a.out32_off + gcol;
+                if (nv >= 4 && ((a.out32_pitch | a.out32_off) & 3) == 0) *reinterpret_cast<float4*>(o) = v;
+                else { o[0] = v.x; if (nv > 1) o[1] = v.y; if (nv > 2) o[2] = v.z; if (nv > 3) o[3] = v.w; }
+            }
+            if (a.out16) {
+                // saturate instead of overflowing to inf (activations here are O(10); this is a guard, not a code path)
+                const float lim = 65504.f;
+                __half2 h2[2] = {__floats2half2_rn(fminf(fmaxf(v.x, -lim), lim), fminf(fmaxf(v.y, -lim), lim)),
+                                 __floats2half2_rn(fminf(fmaxf(v.z, -lim), lim), fminf(fmaxf(v.w, -lim), lim))};
+                __half* o = a.out16 + (a.out16_dense ? d : ur) * a.out16_pitch + a.out16_off + gcol;
+                if (nv >= 4) *reinterpret_cast<uint2*>(o) = *reinterpret_cast<uint2*>(h2);
+                else { o[0] = __low2half(h2[0]); if (nv > 1) o[1] = __high2half(h2[0]); if (nv > 2) o[2] = __low2half(h2[1]); }
+            }
+        }
+    }
+    if (threadIdx.x == 0) tl.end();
+    if (warp == 0 && lane == 0) TR(2);
 }
 
 // 7x7 neighbourhood of the 2-channel flow as GEMM rows (the motion encoder's convf1, gru.py:50,57, becomes a 1x1 convolution):
@@ -279,6 +236,28 @@ flow_im2col_kernel(const float* __restrict__ coords1, const float* __restrict__ 
     }
 }
 
+template <int N>
+int launch_conv(const CUtensorMap& map_a, const CUtensorMap& map_w, const ConvArgs& a, int tiles, int slices, int smem_bytes,
+                cudaStream_t stream) {
+    static bool configured = false;
+    if (!configured) {
+        MACVO_CUDA_TRY(cudaFuncSetAttribute(conv_tc_kernel<N>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_MAX));
+        configured = true;
+    }
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(tiles, slices);
+    cfg.blockDim = dim3(TC_THREADS);
+    cfg.dynamicSmemBytes = smem_bytes;
+    cfg.stream = stream;
+    cudaLaunchAttribute attrs[1];
+    attrs[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attrs[0].val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = attrs;
+    cfg.numAttrs = 1;
+    MACVO_CUDA_TRY(cudaLaunchKernelEx(&cfg, conv_tc_kernel<N>, map_a, map_w, a));
+    return MACVO_OK;
+}
+
 }  // namespace
 
 static Timeline g_timeline = {nullptr, 0, -1};
@@ -307,71 +286,51 @@ extern "C" int macvo_conv_tc(const void* in_rows, int in_channels, int in_dense,
     a.in_dense = in_dense;
     a.batch = batch; a.height = height; a.width = width; a.wp = width + 4;
     a.m_rows = in_dense ? batch * height * width : macvo_rows::padded_pixels(batch, height, width, 0);
-    const int pairs = (a.m_rows + 2 * TILE_M - 1) / (2 * TILE_M);
-    // slices of output channels: as many CTA pairs as fit one wave of the 148 SMs, every slice a multiple of 32 columns (<= 256)
+    const int tiles = (a.m_rows + TILE_M - 1) / TILE_M;
+    int dev = 0, sms = 0;
+    MACVO_CUDA_TRY(cudaGetDevice(&dev));
+    MACVO_CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    // slices of output channels: as many CTAs as fit one wave of the SMs, every slice a multiple of 32 columns (<= 256)
     int slices = 1;
     for (int s = 1; s <= 8; ++s)
-        if (n_pad % (32 * s) == 0 && n_pad / s <= 256 && (2 * pairs * s <= 148 || n_pad / slices > 256)) slices = s;
-    a.n_cta = n_pad / slices;
-    if (a.n_cta > 256) return MACVO_E_UNSUPPORTED;
-    a.tmem_cols = 32;
-    while (a.tmem_cols < a.n_cta) a.tmem_cols *= 2;
-    const int tpg = a.taps == 9 ? 3 : 1;
-    const int slot_bytes = A_BYTES + tpg * (a.n_cta / 2) * 128;
+        if (n_pad % (32 * s) == 0 && n_pad / s <= 256 && (tiles * s <= sms || n_pad / slices > 256)) slices = s;
+    const int n_cta = n_pad / slices;
+    if (n_cta > 256) return MACVO_E_UNSUPPORTED;
+    const int slot_bytes = A_BYTES + n_cta * 128;
     a.slots = (SMEM_MAX - 2048) / slot_bytes;
     if (a.slots > 8) a.slots = 8;
-    if (a.slots < 2 || a.slots * slot_bytes < TILE_M * a.n_cta * 4) return MACVO_E_UNSUPPORTED;    // epilogue staging reuses the ring
+    if (a.slots < 2 || a.slots * slot_bytes < TILE_M * n_cta * 4) return MACVO_E_UNSUPPORTED;    // epilogue staging reuses the ring
     const int smem_bytes = a.slots * slot_bytes + 512 + 1024;
     a.relu = relu; a.n_valid = n_valid; a.bias = bias;
     a.out16 = static_cast<__half*>(out16); a.out16_pitch = out16_pitch; a.out16_off = out16_offset; a.out16_dense = out16_dense;
     a.out32 = out32; a.out32_pitch = out32_pitch; a.out32_off = out32_offset; a.out32_planes = out32_planes;
-    a.idesc = make_idesc_f16(2 * TILE_M, a.n_cta);
     a.tl = g_timeline;
     a.trace = g_conv_trace;
     CUtensorMap map_a, map_w;
     const uint64_t in_rows_total = in_dense ? (uint64_t)a.m_rows : (uint64_t)macvo_rows::alloc_rows(batch, height, width, 0);
-    if (!make_map_2d(&map_a, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, in_rows, in_channels, in_rows_total, (uint64_t)in_channels * 2, BLOCK_K, A_ROWS))
+    if (!make_map_2d(&map_a, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, in_rows, in_channels, in_rows_total, (uint64_t)in_channels * 2, BLOCK_K, TILE_M))
         return MACVO_E_DRIVER;
-    // filters (n_pad, taps * C) as the 3-D view (k within the row, n, dx): box = 64 channels x n_cta / 2 rows x the group's taps
-    {
-        PFN_encodeTiled enc = get_encode_fn();
-        if (!enc) return MACVO_E_DRIVER;
-        const uint64_t kk = (uint64_t)a.taps * in_channels;
-        cuuint64_t dims[3] = {kk, (cuuint64_t)n_pad, (cuuint64_t)tpg};
-        cuuint64_t strides[2] = {kk * 2, (cuuint64_t)in_channels * 2};
-        cuuint32_t box[3] = {BLOCK_K, (cuuint32_t)(a.n_cta / 2), (cuuint32_t)tpg};
-        cuuint32_t estr[3] = {1, 1, 1};
-        if (enc(&map_w, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, const_cast<void*>(weights), dims, strides, box, estr,
-                CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-            return MACVO_E_DRIVER;
+    // filters (n_pad, taps * C): box = 64 channels of one tap x the slice's n_cta rows
+    const uint64_t kk = (uint64_t)a.taps * in_channels;
+    if (!make_map_2d(&map_w, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, weights, kk, n_pad, kk * 2, BLOCK_K, n_cta)) return MACVO_E_DRIVER;
+    cudaStream_t st = as_stream(stream);
+    switch (n_cta) {
+        case 32: return launch_conv<32>(map_a, map_w, a, tiles, slices, smem_bytes, st);
+        case 64: return launch_conv<64>(map_a, map_w, a, tiles, slices, smem_bytes, st);
+        case 96: return launch_conv<96>(map_a, map_w, a, tiles, slices, smem_bytes, st);
+        case 128: return launch_conv<128>(map_a, map_w, a, tiles, slices, smem_bytes, st);
+        case 160: return launch_conv<160>(map_a, map_w, a, tiles, slices, smem_bytes, st);
+        case 192: return launch_conv<192>(map_a, map_w, a, tiles, slices, smem_bytes, st);
+        case 224: return launch_conv<224>(map_a, map_w, a, tiles, slices, smem_bytes, st);
+        default: return launch_conv<256>(map_a, map_w, a, tiles, slices, smem_bytes, st);
     }
-    static bool configured = false;
-    if (!configured) {
-        MACVO_CUDA_TRY(cudaFuncSetAttribute(conv_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_MAX));
-        configured = true;
-    }
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(2 * pairs, slices);
-    cfg.blockDim = dim3(THREADS);
-    cfg.dynamicSmemBytes = smem_bytes;
-    cfg.stream = as_stream(stream);
-    cudaLaunchAttribute attrs[2];
-    attrs[0].id = cudaLaunchAttributeClusterDimension;
-    attrs[0].val.clusterDim.x = 2; attrs[0].val.clusterDim.y = 1; attrs[0].val.clusterDim.z = 1;
-    attrs[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attrs[1].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attrs;
-    cfg.numAttrs = 2;
-    MACVO_CUDA_TRY(cudaLaunchKernelEx(&cfg, conv_tc_kernel, map_a, map_w, a));
-    return MACVO_OK;
 }
 
 extern "C" int macvo_flow_im2col(const float* coords1, const float* coords0, void* rows, float* mf32, void* mf16_rows, int batch,
                                  int height, int width, void* stream) {
     if (!coords1 || !coords0 || !rows || batch <= 0 || height <= 0 || width <= 0) return MACVO_E_ARG;
     const long long total = (long long)batch * height * width * 32;
-    const int blocks = (int)((total + 255) / 256 < 148 * 8 ? (total + 255) / 256 : 148 * 8);
+    const int blocks = (int)((total + 255) / 256 < 132 * 8 ? (total + 255) / 256 : 132 * 8);
     flow_im2col_kernel<<<blocks, 256, 0, as_stream(stream)>>>(coords1, coords0, static_cast<__half*>(rows), mf32,
                                                               static_cast<__half*>(mf16_rows), batch, height, width);
     MACVO_LAUNCH_CHECK();

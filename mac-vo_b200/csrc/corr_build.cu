@@ -6,7 +6,7 @@ size_t macvo_corr_tc_workspace_bytes(int batch, int dim, int n, int passes);
 int macvo_corr_build_tc(const float* f1, const float* f2, float* corr, int batch, int dim, int n, int passes, int kmajor,
                         void* workspace, size_t workspace_bytes, cudaStream_t st);
 
-extern "C" const char* macvo_b200_version(void) { return "macvo_b200 0.1.0 sm_100a"; }
+extern "C" const char* macvo_b200_version(void) { return "macvo_b200 0.1.0 sm_90a"; }
 
 extern "C" size_t macvo_corr_workspace_bytes(int batch, int dim, int n, int mode) {
     if (batch <= 0 || dim <= 0 || n <= 0) return 0;

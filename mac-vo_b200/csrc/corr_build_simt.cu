@@ -5,7 +5,7 @@
 // Both operands arrive "MN-major" (token index contiguous), i.e. C = F1^T F2, so global loads are
 // coalesced along the token axis for both tiles. 128x128 output tile per CTA, 8x8 per thread, K-step 16.
 // This kernel is the reference-accuracy arm: true fp32 FMA accumulation, any N and D. It is
-// compute-bound (~116 flop/B, SURVEY.md §7.3); the roofline kernel is corr_build_tc.cu (tcgen05).
+// compute-bound (~116 flop/B, SURVEY.md §7.3); the roofline kernel is corr_build_tc.cu (wgmma).
 #include "common.cuh"
 
 namespace {

@@ -1,4 +1,4 @@
-// (a3) all-pairs correlation volume on the 5th-generation tensor cores (tcgen05 / TMEM / TMA), sm_100a.
+// (a3) all-pairs correlation volume on the Hopper tensor cores (wgmma, TMA, mbarrier), sm_90a.
 //
 // Replaces MemoryEncoder.corr (Module/Network/FlowFormer/core/encoder.py:256-275; one cuBLAS bmm in the
 // reference):  corr[b, i, j] = sum_d f1[b, d, i] * f2[b, d, j],  output (B, N, N) fp32 — 184 MB per
@@ -7,61 +7,38 @@
 //
 // fp32-class accuracy on fp16 tensor cores (MACVO_CORR_TC_3XF16): every operand is scaled by 2^6 and split
 //     x = hi + lo,  hi = fp16(x),  lo = fp16(x - hi)          (|x - hi - lo| <~ 2^-22 |x|)
-// and  hi*hi + hi*lo + lo*hi  is accumulated in fp32 in TMEM, rescaled by 2^-12 in the epilogue (the
+// and  hi*hi + hi*lo + lo*hi  is accumulated in fp32 registers, rescaled by 2^-12 in the epilogue (the
 // power-of-two scale keeps `lo` out of the fp16 subnormal range for |x| > 4e-3; fp16(x * 64) stays finite
 // for |x| < 1023). MACVO_CORR_TC_1XF16 keeps only hi*hi, unscaled (exact for the MACVO_Fast configuration
-// whose encoder already emits fp16 features).
+// whose encoder already emits fp16 features). MACVO_CORR_TC_TF32 runs one wgmma kind tf32 pass straight over
+// the fp32 K-major features (no pre-pass, no workspace).
 //
-// v1 of this kernel (both operands from shared memory, SS-mode MMA, one CTA per tile) measured 72 us at
-// 640x480: ncu showed the tensor pipe only 50 % active — bound by the L2->SM operand stream (256 KB per
-// 64 KB of output) and by shared-memory bandwidth (8 KB of operand reads per 64-cycle MMA).
-// This version moves A out of shared memory and shares B across a CTA pair:
-//
-//   * A (the 128 query rows of a tile, all K = 256) lives in TENSOR MEMORY (2 x 128 columns, fp16 hi | lo).
-//     When a cluster moves to a new row of tiles the TMA producer pushes the A block through the same
-//     shared-memory ring as 4 extra stages and the MMA thread forwards each stage with tcgen05.cp
-//     (smem -> TMEM, 128x256b); tcgen05.cp / tcgen05.mma execute in issue order, so no further
-//     synchronisation is needed. A then stays put for the whole row (A-stationary) and tcgen05.mma runs in
-//     TS mode (A from TMEM, B from smem) -> half the shared-memory operand reads of SS mode.
-//     (v2 staged A with per-thread global loads + tcgen05.st from the epilogue warps: ncu showed those
-//     warps spending ~35 % of their time in the scattered loads.)
-//   * both operands are pre-split by one small pre-pass into K-major fp16 hi/lo; B is streamed by TMA
-//     (SWIZZLE_128B, 64-wide K slices) through a ring of 16 KB mbarrier-guarded slots. The two CTAs of a
-//     cluster form a tcgen05 CTA PAIR (cta_group::2): one thread of the leader issues 256 x 128 x 16 MMAs
-//     that span both SMs; each CTA keeps its own 128 A rows in its TMEM and stages only HALF of every B
-//     tile (64 key rows) in its shared memory -> per-SM operand ingest and smem operand reads are halved
-//     again (v3, which multicast the full B tile into both CTAs, was bound by exactly those two: its MMA
-//     time and its TMA load time ADDED UP instead of overlapping).
-//   * 320 threads: warp 0 TMA producer, warp 1 MMA issuer (one elected thread), warps 2..9 epilogue
-//     (tcgen05.ld TMEM -> registers -> per-warp smem transpose -> coalesced 128-bit st.global). An event
-//     trace of v4 (4 epilogue warps, smem-staged TMA stores) showed the epilogue taking 2.6-3.5 us per step
-//     against 1.7 us of MMA work: K = 256 is so short that draining the accumulator is the critical path,
-//     so the drain is spread over 8 warps. Double-buffered TMEM accumulators (2 x 128 columns) overlap it
-//     with the next tile's MMAs.
-//   * Persistent: every cluster owns a contiguous run of (batch, row-pair, column) steps; M/N edges are
-//     handled by TMA (zero fill on load, clipping on store) and by row guards in the A loader.
+//   * both operands are pre-split by one small pre-pass into K-major fp16 hi/lo and streamed by TMA
+//     (SWIZZLE_128B, 64-wide K slices) through a ring of mbarrier-guarded stages: one stage = one 64-channel
+//     k-block of the 128 query rows (A) and the 128 key rows (B), hi and lo.
+//   * 288 threads: warps 0..7 = two consumer warpgroups, each owning 64 query rows of the 128 x 128 output tile
+//     (m64n128k16 wgmma, 64 fp32 accumulators per thread); warp 8 = TMA producer.
+//   * Persistent: CTA c takes tiles c, c + grid, ...; the producer runs up to a whole ring ahead, so the next
+//     tile's operands stream in while the consumers write the previous tile (K = 256 is so short that the
+//     output stores, not the MMAs, are the critical path). M/N edges: TMA zero fill on load, row guards on store.
 #include "tc_common.cuh"
 #include <cuda_fp16.h>
-#include <cstdlib>
 
 namespace {
 
-constexpr int BLOCK_M = 128, BLOCK_N = 128, BLOCK_K = 64, UMMA_K = 16;
-constexpr int SLOTS = 10;                                    // shared-memory ring of 16 KB slots
-constexpr int SLOT_BYTES = BLOCK_M * BLOCK_K * 2;            // 16 KB: one A k-block half (128 rows x 64 fp16)
-constexpr int B_HALF_BYTES = (BLOCK_N / 2) * BLOCK_K * 2;    // 8 KB: this CTA's 64 key rows x 64 fp16 (hi or lo)
-constexpr int NUM_EPI_WARPS = 8;                             // 2 per TMEM lane quarter: each drains 64 of the 128 columns
-constexpr int EPI_COLS = BLOCK_N / 2;                        // 64 fp32 columns per epilogue warp
-constexpr int EPI_WARP_BYTES = 32 * EPI_COLS * 4;            // 8 KB transpose buffer per epilogue warp
-constexpr int SMEM_EPI_BYTES = NUM_EPI_WARPS * EPI_WARP_BYTES;  // 64 KB
-constexpr int SMEM_BAR_BYTES = 512;
-constexpr int SMEM_TOTAL = SLOTS * SLOT_BYTES + SMEM_EPI_BYTES + SMEM_BAR_BYTES + 1024;  // + alignment slack
-constexpr int THREADS = 32 * (2 + NUM_EPI_WARPS);
-constexpr int TMEM_COLS = 512;            // [0,256): 2 accumulators x 128 | [256,384): A hi | [384,512): A lo
-constexpr int TMEM_A_HI = 256, TMEM_A_LO = 384;
-constexpr int KMAX = 256;                 // A-stationary capacity: K fp16 = 128 TMEM columns per half
+constexpr int BLOCK_M = 128, BLOCK_N = 128, BLOCK_K = 64;
+constexpr int SUB_BYTES = 128 * 128;                         // 16 KB: 128 rows x 128 B (64 fp16 | 32 fp32)
 constexpr float SPLIT_SCALE = 64.f;       // 2^6 on both operands
 constexpr float SPLIT_UNSCALE = 1.f / 4096.f;
+
+// PASSES 3: fp16 hi*hi + hi*lo + lo*hi (fp32-class)    1: fp16 hi*hi    2: ONE tf32 pass over the fp32 K-major features,
+// whose 64-channel k-block is two 32-channel (128 B) sub-tiles per operand
+template <int PASSES> struct CorrCfg {
+    static constexpr int SUBS = PASSES == 1 ? 1 : 2;         // sub-tiles per operand and k-block
+    static constexpr int STAGE_BYTES = 2 * SUBS * SUB_BYTES; // [A sub-tiles | B sub-tiles]
+    static constexpr int STAGES = PASSES == 1 ? 6 : 3;
+    static constexpr int SMEM = STAGES * STAGE_BYTES + 256 + 1024;   // + barriers + alignment slack
+};
 
 // ---- kernel 1: operand pre-pass: fp32 (B, D, N) -> fp16 hi / lo (B, N, D), scaled (both maps, one launch) ----
 __global__ void __launch_bounds__(256)
@@ -136,325 +113,128 @@ split_kmajor_kernel(const float* __restrict__ f1, const float* __restrict__ f2, 
     }
 }
 
-__device__ __forceinline__ void stg128(float* p, float4 v, int mode, uint64_t policy) {
-    if (mode == 0)
-        asm volatile("st.global.L2::cache_hint.v4.f32 [%0], {%1, %2, %3, %4}, %5;"
-                     ::"l"(p), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w), "l"(policy) : "memory");
-    else if (mode == 2)
-        asm volatile("st.global.cs.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(p), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w) : "memory");
-    else
-        *reinterpret_cast<float4*>(p) = v;
-}
-
 // ---- kernel 2 -----------------------------------------------------------------------------------------------
-// PASSES 3: fp16 hi*hi + hi*lo + lo*hi (fp32-class)    1: fp16 hi*hi    2: ONE kind::tf32 pass straight over the fp32
-// K-major features (no operand pre-pass, no workspace): map_a_hi / map_b_hi are fp32 maps with 32-element (128 B) boxes,
-// the "lo" half of every 16 KB ring slot carries the NEXT 32 channels instead of the low-order fp16 part, A occupies
-// TMEM columns [256, 512) as 256 fp32 values per lane, and a 64-channel k-block is 8 MMAs of K = 8 (12 in mode 3).
 template <int PASSES>
-__global__ void __launch_bounds__(THREADS, 1)
+__global__ void __launch_bounds__(TC_THREADS, 1)
 corr_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ CUtensorMap map_a_lo,
                const __grid_constant__ CUtensorMap map_b_hi, const __grid_constant__ CUtensorMap map_b_lo,
-               float* __restrict__ corr, int batch, int n, int dim, int dbg, unsigned long long* __restrict__ trace) {
+               float* __restrict__ corr, int batch, int n, int dim) {
+    using C = CorrCfg<PASSES>;
+    constexpr bool TF32 = PASSES == 2;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    uint8_t* smem_epi = smem + SLOTS * SLOT_BYTES;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem_epi + SMEM_EPI_BYTES);
-    // barrier slots: full[SLOTS] (leader CTA only), empty[SLOTS], tmem_full[2], tmem_empty[2] (leader only), TMEM base
-    const uint32_t bar_full = smem_u32(bars), bar_empty = bar_full + 8 * SLOTS;
-    const uint32_t bar_tfull = bar_empty + 8 * SLOTS, bar_tempty = bar_tfull + 16;
-    uint32_t* tmem_base_slot = reinterpret_cast<uint32_t*>(bars + 2 * SLOTS + 4);
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t rank = cluster_ctarank();                    // 0 = leader (issues every MMA of the pair), 1 = peer
-    const bool leader = rank == 0;
-    // profiling aid (dbg bit 3): timestamped events of cluster 0 -> trace[cta][role][event] (ns)
-    int tr_n = 0;
-    auto TR = [&](int role, int tag) {
-        if (trace != nullptr && (blockIdx.x >> 1) == 0 && tr_n < 512) {
-            unsigned long long t;
-            asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-            trace[(((blockIdx.x & 1) * 4 + role) * 512 + tr_n) * 2] = t;
-            trace[(((blockIdx.x & 1) * 4 + role) * 512 + tr_n) * 2 + 1] = tag;
-            ++tr_n;
-        }
-    };
-    const int cluster_id = blockIdx.x >> 1, num_clusters = gridDim.x >> 1;
-    const int mt = ceil_div(n, BLOCK_M), nt = ceil_div(n, BLOCK_N), prows = (mt + 1) / 2, kblocks = dim / BLOCK_K;
-    const int total_steps = batch * prows * nt;
-    // static contiguous runs (column index fastest -> A stays put for up to a whole row of tiles)
-    const int s_begin = (int)((long long)total_steps * cluster_id / num_clusters);
-    const int s_end = (int)((long long)total_steps * (cluster_id + 1) / num_clusters);
-    // a step is (row = b * prows + prow, column tile) = one 256 x 128 output block of the CTA pair
-    const int row_begin = s_begin / nt, col_begin = s_begin - row_begin * nt;
-    constexpr bool TF32 = PASSES == 2;
-    constexpr int A_SLOTS_PER_KB = PASSES == 1 ? 1 : 2;        // A k-block: hi slot (+ lo slot)  |  tf32: channels [0,32) + [32,64)
-    constexpr uint32_t A_SLOT_TX = 2 * SLOT_BYTES;              // both CTAs deliver 16 KB
-    constexpr uint32_t B_SLOT_TX = 2 * (PASSES == 1 ? 1 : 2) * B_HALF_BYTES;
+    const uint32_t bar_full = smem_u32(smem + C::STAGES * C::STAGE_BYTES), bar_empty = bar_full + 8 * C::STAGES;
+    const int warp = threadIdx.x >> 5;
+    const int mt = ceil_div(n, BLOCK_M), nt = ceil_div(n, BLOCK_N), kblocks = dim / BLOCK_K;
+    const int tiles = batch * mt * nt;
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < SLOTS; ++s) { mbar_init(bar_full + 8 * s, 1); mbar_init(bar_empty + 8 * s, 1); }
-        for (int s = 0; s < 2; ++s) { mbar_init(bar_tfull + 8 * s, 1); mbar_init(bar_tempty + 8 * s, NUM_EPI_WARPS); }   // 4 warps x 2 CTAs per accumulator
+        for (int s = 0; s < C::STAGES; ++s) { mbar_init(bar_full + 8 * s, 1); mbar_init(bar_empty + 8 * s, 2); }
         fence_barrier_init();
+        prefetch_tmap(&map_a_hi); prefetch_tmap(&map_b_hi);
     }
-    if (warp == 1) tmem_alloc(smem_u32(tmem_base_slot), TMEM_COLS);   // cta_group::2: the same warp of both CTAs
-    tc_fence_before();
     __syncthreads();
-    cluster_sync_all();                       // peer barriers are initialised before any remote arrive / 2-CTA copy
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_base_slot;
 
-    if (warp == 0) {
-        // ===================== TMA producer (both CTAs; completion is signalled on the leader's barriers) ==========
+    if (warp == TC_PRODUCER_WARP) {
+        // ===================== TMA producer =====================
         if (elect_one()) {
-            // programmatic dependent launch: everything above (barrier init, TMEM allocation, cluster sync) overlapped the
-            // tail of the operand pre-pass; its fp16 operands are only touched from here on
+            // programmatic dependent launch: the set-up above overlapped the tail of the operand pre-pass
             asm volatile("griddepcontrol.wait;" ::: "memory");
-            int slot = 0; uint32_t phase = 0;
-            int row = row_begin, col = col_begin;
-            bool new_row = true;
-            for (int s = s_begin; s < s_end; ++s) {
-                const int b = row / prows, m_tile = 2 * (row - b * prows) + (int)rank;
-                if (new_row) {
-                    // this CTA's 128 query rows, K-major: one 16 KB slot per (k-block, hi | lo)
-                    for (int kb = 0; kb < kblocks; ++kb) {
-                        for (int h = 0; h < A_SLOTS_PER_KB; ++h) {
-                            mbar_wait(bar_empty + 8 * slot, phase ^ 1);
-                            const uint32_t full = bar_full + 8 * slot;
-                            if (leader) mbar_expect_tx(full, A_SLOT_TX);
-                            if (TF32)
-                                tma_load_3d_2cta(smem_u32(smem + slot * SLOT_BYTES), &map_a_hi, full,
-                                                 kb * BLOCK_K + h * 32, m_tile * BLOCK_M, b);
-                            else
-                                tma_load_3d_2cta(smem_u32(smem + slot * SLOT_BYTES), h == 0 ? &map_a_hi : &map_a_lo, full,
-                                                 kb * BLOCK_K, m_tile * BLOCK_M, b);
-                            if (++slot == SLOTS) { slot = 0; phase ^= 1; }
-                        }
-                    }
-                }
-                // this CTA's half (64 key rows) of the B tile: [hi 8 KB | lo 8 KB] per k-block slot
+            int stage = 0; uint32_t phase = 0;
+            for (int t = blockIdx.x; t < tiles; t += gridDim.x) {
+                const int b = t / (mt * nt), rem = t - b * mt * nt, m0 = (rem / nt) * BLOCK_M, n0 = (rem % nt) * BLOCK_N;
                 for (int kb = 0; kb < kblocks; ++kb) {
-                    mbar_wait(bar_empty + 8 * slot, phase ^ 1);
-                    TR(0, 100 + slot);
-                    const uint32_t sb = smem_u32(smem + slot * SLOT_BYTES);
-                    const uint32_t full = bar_full + 8 * slot;
-                    if (leader) mbar_expect_tx(full, B_SLOT_TX);
-                    const int brow = col * BLOCK_N + (int)rank * (BLOCK_N / 2);
-                    tma_load_3d_2cta(sb, &map_b_hi, full, kb * BLOCK_K, brow, b);
-                    if (PASSES == 3) tma_load_3d_2cta(sb + B_HALF_BYTES, &map_b_lo, full, kb * BLOCK_K, brow, b);
-                    if (TF32) tma_load_3d_2cta(sb + B_HALF_BYTES, &map_b_hi, full, kb * BLOCK_K + 32, brow, b);
-                    TR(0, 200 + slot);
-                    if (++slot == SLOTS) { slot = 0; phase ^= 1; }
-                }
-                new_row = false;
-                if (++col == nt) { col = 0; ++row; new_row = true; }
-            }
-        }
-    } else if (warp == 1) {
-        // ===================== MMA issuer: leader CTA only, cta_group::2, TS mode =====================
-        if (leader) {
-            constexpr uint32_t idesc = TF32 ? make_idesc_tf32(2 * BLOCK_M, BLOCK_N)
-                                            : make_idesc_f16(2 * BLOCK_M, BLOCK_N);      // M = 256 across the pair
-            int slot = 0; uint32_t phase = 0;
-            int acc = 0; uint32_t acc_phase = 0;
-            int col = col_begin;
-            bool new_row = true;
-            for (int s = s_begin; s < s_end; ++s) {
-                if (new_row) {
-                    // forward the A block smem -> TMEM in both CTAs; issue order keeps it behind the previous row's MMAs
-                    for (int kb = 0; kb < kblocks; ++kb) {
-                        for (int h = 0; h < A_SLOTS_PER_KB; ++h) {
-                            mbar_wait(bar_full + 8 * slot, phase);
-                            tc_fence_after();
-                            if (elect_one()) {
-                                const uint64_t adesc = make_kmajor_sw128_desc(smem_u32(smem + slot * SLOT_BYTES));
-#pragma unroll
-                                for (int k = 0; k < BLOCK_K / UMMA_K; ++k) {
-                                    const uint64_t koff = (uint64_t)((k * UMMA_K * 2) >> 4);      // 32 B per copy: 16 fp16 | 8 fp32
-                                    if (TF32) {
-                                        tmem_cp_128x256b(tmem_base + TMEM_A_HI + kb * BLOCK_K + h * 32 + k * 8, adesc + koff);
-                                    } else {
-                                        const uint32_t acol = (uint32_t)((kb * BLOCK_K + k * UMMA_K) >> 1);
-                                        tmem_cp_128x256b(tmem_base + (h == 0 ? TMEM_A_HI : TMEM_A_LO) + acol, adesc + koff);
-                                    }
-                                }
-                                umma_commit_mc(bar_empty + 8 * slot, 3);
-                            }
-                            __syncwarp();
-                            if (++slot == SLOTS) { slot = 0; phase ^= 1; }
+                    mbar_wait(bar_empty + 8 * stage, phase ^ 1);
+                    const uint32_t full = bar_full + 8 * stage, sa = smem_u32(smem + stage * C::STAGE_BYTES);
+                    const uint32_t sb = sa + C::SUBS * SUB_BYTES;
+                    mbar_expect_tx(full, C::STAGE_BYTES);
+                    if (TF32) {
+                        tma_load_3d(sa, &map_a_hi, full, kb * BLOCK_K, m0, b);
+                        tma_load_3d(sa + SUB_BYTES, &map_a_hi, full, kb * BLOCK_K + 32, m0, b);
+                        tma_load_3d(sb, &map_b_hi, full, kb * BLOCK_K, n0, b);
+                        tma_load_3d(sb + SUB_BYTES, &map_b_hi, full, kb * BLOCK_K + 32, n0, b);
+                    } else {
+                        tma_load_3d(sa, &map_a_hi, full, kb * BLOCK_K, m0, b);
+                        tma_load_3d(sb, &map_b_hi, full, kb * BLOCK_K, n0, b);
+                        if (PASSES == 3) {
+                            tma_load_3d(sa + SUB_BYTES, &map_a_lo, full, kb * BLOCK_K, m0, b);
+                            tma_load_3d(sb + SUB_BYTES, &map_b_lo, full, kb * BLOCK_K, n0, b);
                         }
                     }
+                    if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
                 }
-                mbar_wait(bar_tempty + 8 * acc, acc_phase ^ 1);              // both CTAs' epilogues drained this accumulator
-                if (lane == 0) TR(1, 300 + acc);
-                tc_fence_after();
-                const uint32_t tmem_d = tmem_base + acc * BLOCK_N;
-                for (int kb = 0; kb < kblocks; ++kb) {
-                    mbar_wait(bar_full + 8 * slot, phase);
-                    tc_fence_after();
-                    if (lane == 0) TR(1, 400 + slot);
-                    if (elect_one()) {
-                        const uint32_t sb = smem_u32(smem + slot * SLOT_BYTES);
-                        const uint64_t b_hi = make_kmajor_sw128_desc(sb), b_lo = make_kmajor_sw128_desc(sb + B_HALF_BYTES);
-#pragma unroll
-                        for (int k = 0; k < BLOCK_K / UMMA_K; ++k) {
-                            const uint64_t koff = (uint64_t)((k * UMMA_K * 2) >> 4);          // +32 B per K step in the atom
-                            const uint32_t acol = (uint32_t)((kb * BLOCK_K + k * UMMA_K) >> 1);   // 2 fp16 per TMEM column
-                            if (dbg & 2) continue;                                   // profiling aid: no MMA
-                            if (TF32) {          // channels kb*64 + [8k, 8k+8) from the first half slot, + 32 from the second
-                                const uint32_t a0 = tmem_base + TMEM_A_HI + kb * BLOCK_K + k * 8;
-                                umma_tf32_ts(tmem_d, a0, b_hi + koff, idesc, (kb | k) != 0);
-                                umma_tf32_ts(tmem_d, a0 + 32, b_lo + koff, idesc, 1u);
-                            } else if (PASSES == 3) {   // small cross terms first, the dominant hi*hi product last
-                                umma_f16_ts(tmem_d, tmem_base + TMEM_A_LO + acol, b_hi + koff, idesc, (kb | k) != 0);
-                                umma_f16_ts(tmem_d, tmem_base + TMEM_A_HI + acol, b_lo + koff, idesc, 1u);
-                                umma_f16_ts(tmem_d, tmem_base + TMEM_A_HI + acol, b_hi + koff, idesc, 1u);
-                            } else {
-                                umma_f16_ts(tmem_d, tmem_base + TMEM_A_HI + acol, b_hi + koff, idesc, (kb | k) != 0);
-                            }
-                        }
-                        umma_commit_mc(bar_empty + 8 * slot, 3);             // slot reusable in BOTH CTAs once these retire
-                        if (kb == kblocks - 1) umma_commit_mc(bar_tfull + 8 * acc, 3);   // accumulator complete, both CTAs
-                    }
-                    __syncwarp();
-                    if (++slot == SLOTS) { slot = 0; phase ^= 1; }
-                }
-                if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-                new_row = false;
-                if (++col == nt) { col = 0; new_row = true; }
             }
         }
     } else {
-        // ===================== epilogue: TMEM -> registers -> smem transpose -> coalesced global stores ==========
-        // 8 warps in two groups of four; group g owns accumulator g, i.e. every second step, so the TMEM drain of
-        // one tile (TMEM read port) overlaps the global stores of the previous one (LSU). Warp w covers TMEM
-        // lanes [32 (w & 3), +32) and drains the 128 columns in two halves of 64.
-        // tcgen05.ld hands every lane one output ROW. Storing that directly costs 32 distinct cache lines per
-        // warp instruction (an event trace showed those stores saturating the LSU queue and delaying the TMA
-        // producer's issue slots by ~1 us per step), so the warp transposes each 32 x 64 block through a private
-        // 8 KB XOR-swizzled shared-memory buffer and writes 2 rows x 256 contiguous bytes per instruction.
-        const int quarter = warp & 3;
-        const int group = (warp - 2) >> 2;
-        // L2 policy of the output stores: evict-first (the volume is consumed once, by PatchEmbed / the lookups, and does not fit
-        // the 126 MB L2 anyway). Measured: no effect at N = 4800 (the kernel is not write-back bound), 2-3 % at N = 14400.
-        const int store_mode = (dbg >> 8) & 3;                  // 0: evict-first policy (default)  1: plain  2: st.global.cs
-        uint64_t store_policy = 0;
-        asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(store_policy));
+        // ===================== consumers: wgmma over this warpgroup's 64 rows, then the stores =====================
+        const int wg = warp >> 2, lane = threadIdx.x & 31;
         const float unscale = PASSES == 3 ? SPLIT_UNSCALE : 1.f;
-        const uint32_t tb = smem_u32(smem_epi + (warp - 2) * EPI_WARP_BYTES);
-        const int acc = group;
-        uint32_t acc_phase = 0;
-        int row = row_begin, col = col_begin + group;
-        while (col >= nt) { col -= nt; ++row; }
-        for (int s = s_begin + group; s < s_end; s += 2) {
-            const int b = row / prows, m_tile = 2 * (row - b * prows) + (int)rank;
-            const int orow0 = m_tile * BLOCK_M + quarter * 32;
-            mbar_wait(bar_tfull + 8 * acc, acc_phase);
-            tc_fence_after();
-            if (warp == 2 && lane == 0) TR(2, 500 + acc);
-            // drain the warp's whole 32 x 128 accumulator slice into registers first and hand the accumulator back at once
-            // (an event trace showed it being held 1.5 us — the smem transpose + stores of the first half — while the
-            // MMAs of the tile after next were waiting for it); the transposes / stores then overlap the next MMAs.
-            uint32_t r[4][32];
-            if (dbg & 64) {                               // profiling aid: no TMEM drain, no transposes, no stores
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) mbar_arrive_remote(bar_tempty + 8 * acc, 0);
-                acc_phase ^= 1;
-                col += 2;
-                while (col >= nt) { col -= nt; ++row; }
-                continue;
-            }
-            {
-                const uint32_t taddr = tmem_base + ((uint32_t)(quarter * 32) << 16) + acc * BLOCK_N;
-                tmem_ld_32x32b_x32(taddr, r[0]);
-                tmem_ld_32x32b_x32(taddr + 32, r[1]);
-                tmem_ld_32x32b_x32(taddr + 64, r[2]);
-                tmem_ld_32x32b_x32(taddr + 96, r[3]);
-                tmem_ld_wait();
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) mbar_arrive_remote(bar_tempty + 8 * acc, 0);
-                if (warp == 2 && lane == 0) TR(2, 600 + acc);
-            }
+        float acc[BLOCK_N / 2];
+        int stage = 0; uint32_t phase = 0;
+        for (int t = blockIdx.x; t < tiles; t += gridDim.x) {
+            const int b = t / (mt * nt), rem = t - b * mt * nt, m0 = (rem / nt) * BLOCK_M, n0 = (rem % nt) * BLOCK_N;
+            for (int kb = 0; kb < kblocks; ++kb) {
+                mbar_wait(bar_full + 8 * stage, phase);
+                const uint32_t sa = smem_u32(smem + stage * C::STAGE_BYTES) + wg * 64 * 128, sb = sa - wg * 64 * 128 + C::SUBS * SUB_BYTES;
+                const uint64_t a0 = make_kmajor_sw128_desc(sa), a1 = make_kmajor_sw128_desc(sa + SUB_BYTES);
+                const uint64_t b0 = make_kmajor_sw128_desc(sb), b1 = make_kmajor_sw128_desc(sb + SUB_BYTES);
+                wgmma_fence();
 #pragma unroll
-            for (int h = 0; h < 2; ++h) {
-                // write: row = lane (256 B), 16-byte chunk c stored at c ^ (row & 7)  -> conflict free
-#pragma unroll
-                for (int c = 0; c < 16; ++c) {
-                    float4 v;
-                    v.x = __uint_as_float(r[2 * h + (c >> 3)][4 * (c & 7) + 0]) * unscale;
-                    v.y = __uint_as_float(r[2 * h + (c >> 3)][4 * (c & 7) + 1]) * unscale;
-                    v.z = __uint_as_float(r[2 * h + (c >> 3)][4 * (c & 7) + 2]) * unscale;
-                    v.w = __uint_as_float(r[2 * h + (c >> 3)][4 * (c & 7) + 3]) * unscale;
-                    sts128(tb + lane * 256 + ((c ^ (lane & 7)) << 4), v);
-                }
-                __syncwarp();
-                // read back transposed: instruction i covers rows 2i, 2i+1; 16 lanes x 16 B = one 256-byte row segment
-                const int ocol = col * BLOCK_N + h * EPI_COLS + (lane & 15) * 4;
-                float* dst0 = corr + ((long long)b * n + orow0) * n + ocol;
-                if (!(dbg & 1)) {
-                    // (batching the 16 shared loads ahead of the 16 stores costs 64 more live registers and measured 8 us
-                    // SLOWER — r2_corr_probe_3.log — so loads and stores stay interleaved)
-#pragma unroll
-                    for (int i = 0; i < 16; ++i) {
-                        const int rr = 2 * i + (lane >> 4);
-                        const float4 v = lds128(tb + rr * 256 + (((lane & 15) ^ (rr & 7)) << 4));
-                        if (orow0 + rr < n && ocol < n) stg128(dst0 + (long long)rr * n, v, store_mode, store_policy);   // n % 8 == 0
+                for (int k = 0; k < 4; ++k) {                        // 32 B of the 128-byte row per step: 16 fp16 | 8 fp32
+                    const uint32_t first = (kb | k) != 0;
+                    if (TF32) {              // channels kb*64 + [8k, 8k+8) from the first sub-tile, + 32 from the second
+                        Wgmma<BLOCK_N>::tf32(acc, a0 + 2 * k, b0 + 2 * k, first);
+                        Wgmma<BLOCK_N>::tf32(acc, a1 + 2 * k, b1 + 2 * k, 1u);
+                    } else if (PASSES == 3) {   // small cross terms first, the dominant hi*hi product last
+                        Wgmma<BLOCK_N>::f16(acc, a1 + 2 * k, b0 + 2 * k, first);
+                        Wgmma<BLOCK_N>::f16(acc, a0 + 2 * k, b1 + 2 * k, 1u);
+                        Wgmma<BLOCK_N>::f16(acc, a0 + 2 * k, b0 + 2 * k, 1u);
+                    } else {
+                        Wgmma<BLOCK_N>::f16(acc, a0 + 2 * k, b0 + 2 * k, first);
                     }
                 }
-                __syncwarp();                                             // buffer is reused by the next half
+                wgmma_commit();
+                wgmma_wait<0>();
+                fence_acc(acc);
+                if ((threadIdx.x & 127) == 0) mbar_arrive(bar_empty + 8 * stage);   // this warpgroup is done with the stage
+                if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
             }
-            if (warp == 2 && lane == 0) TR(2, 700 + acc);
-            acc_phase ^= 1;
-            col += 2;
-            while (col >= nt) { col -= nt; ++row; }
+            // fragment -> rows: 4 lanes cover 8 consecutive columns (32 B) of a row; the volume is written once, streaming stores
+            const int r0 = m0 + wg * 64 + (warp & 3) * 16 + (lane >> 2), c0 = n0 + 2 * (lane & 3);
+            float* base = corr + (long long)b * n * n;
+#pragma unroll
+            for (int i = 0; i < BLOCK_N / 2; i += 2) {
+                const int r = r0 + 8 * ((i >> 1) & 1), c = c0 + 8 * (i >> 2);
+                if (r < n && c < n)                                          // n % 8 == 0: c < n implies c + 1 < n
+                    __stcs(reinterpret_cast<float2*>(base + (long long)r * n + c), make_float2(acc[i] * unscale, acc[i + 1] * unscale));
+            }
         }
-    }
-
-    tc_fence_before();
-    __syncthreads();
-    cluster_sync_all();                       // no CTA exits while its peer may still signal / copy into it
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, TMEM_COLS);
     }
 }
 
 // ---- host side ---------------------------------------------------------------------------------------------
 size_t operand_bytes(int batch, int dim, int n) { return ((size_t)batch * n * dim * 2 + 1023) / 1024 * 1024; }
 
-unsigned long long* g_trace = nullptr;
-
 template <int PASSES>
 int launch_main(const CUtensorMap& a_hi, const CUtensorMap& a_lo, const CUtensorMap& b_hi, const CUtensorMap& b_lo,
-                float* m_out, int batch, int n, int dim, int clusters, cudaStream_t st) {
-    MACVO_CUDA_TRY(cudaFuncSetAttribute(corr_tc_kernel<PASSES>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_TOTAL));
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(2 * clusters);
-    cfg.blockDim = dim3(THREADS);
-    cfg.dynamicSmemBytes = SMEM_TOTAL;
-    cfg.stream = st;
-    static const int dbg = getenv("MACVO_B200_CORR_DEBUG") ? atoi(getenv("MACVO_B200_CORR_DEBUG")) : 0;
-    cudaLaunchAttribute attr[2];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    // programmatic dependent launch on the operand pre-pass (bit 32 of MACVO_B200_CORR_DEBUG switches it off)
-    attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[1].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = (dbg & 32) ? 1 : 2;
-    unsigned long long* trace = nullptr;
-    if (dbg & 8) {   // profiling aid: leave the event trace of cluster 0 in a managed buffer and dump it at exit
-        static unsigned long long* tbuf = nullptr;
-        if (!tbuf) { cudaMallocManaged(&tbuf, 2 * 4 * 512 * 2 * sizeof(unsigned long long)); }
-        cudaMemsetAsync(tbuf, 0, 2 * 4 * 512 * 2 * sizeof(unsigned long long), st);
-        trace = tbuf;
-        g_trace = tbuf;
+                float* m_out, int batch, int n, int dim, int ctas, cudaStream_t st) {
+    static bool configured = false;
+    if (!configured) {
+        MACVO_CUDA_TRY(cudaFuncSetAttribute(corr_tc_kernel<PASSES>, cudaFuncAttributeMaxDynamicSharedMemorySize, CorrCfg<PASSES>::SMEM));
+        configured = true;
     }
-    MACVO_CUDA_TRY(cudaLaunchKernelEx(&cfg, corr_tc_kernel<PASSES>, a_hi, a_lo, b_hi, b_lo, m_out, batch, n, dim, dbg, trace));
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(ctas);
+    cfg.blockDim = dim3(TC_THREADS);
+    cfg.dynamicSmemBytes = CorrCfg<PASSES>::SMEM;
+    cfg.stream = st;
+    // programmatic dependent launch on the operand pre-pass
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[0].val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    MACVO_CUDA_TRY(cudaLaunchKernelEx(&cfg, corr_tc_kernel<PASSES>, a_hi, a_lo, b_hi, b_lo, m_out, batch, n, dim));
     return MACVO_OK;
 }
 
@@ -466,24 +246,21 @@ size_t macvo_corr_tc_workspace_bytes(int batch, int dim, int n, int passes) {
 
 int macvo_corr_build_tc(const float* f1, const float* f2, float* corr, int batch, int dim, int n, int passes, int kmajor,
                         void* workspace, size_t workspace_bytes, cudaStream_t st) {
-    if (dim % BLOCK_K != 0 || dim > KMAX || n % 8 != 0) return MACVO_E_UNSUPPORTED;
+    if (dim % BLOCK_K != 0 || n % 8 != 0) return MACVO_E_UNSUPPORTED;
     if (reinterpret_cast<uintptr_t>(corr) & 31) return MACVO_E_ARG;
     int dev = 0, sms = 0;
     MACVO_CUDA_TRY(cudaGetDevice(&dev));
     MACVO_CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    const int mt = ceil_div(n, BLOCK_M), nt = ceil_div(n, BLOCK_N);
-    const int total_steps = batch * ((mt + 1) / 2) * nt;
-    int clusters = sms / 2;
-    if (clusters > total_steps) clusters = total_steps;
-    if (clusters < 1) clusters = 1;
+    const long long tiles = (long long)batch * ceil_div(n, BLOCK_M) * ceil_div(n, BLOCK_N);
+    const int ctas = (int)(tiles < sms ? tiles : sms);                 // one persistent CTA per SM (the ring fills shared memory)
     if (passes == 2) {
-        // kind::tf32: TMA reads the fp32 (B, N, D) features themselves, 32 channels (128 B) per swizzled row
+        // tf32: TMA reads the fp32 (B, N, D) features themselves, 32 channels (128 B) per swizzled row
         if (!kmajor || (reinterpret_cast<uintptr_t>(f1) & 15) || (reinterpret_cast<uintptr_t>(f2) & 15)) return MACVO_E_ARG;
         CUtensorMap m_a, m_b;
         bool ok = make_map_3d(&m_a, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<float*>(f1), dim, n, batch, 32, BLOCK_M);
-        ok = ok && make_map_3d(&m_b, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<float*>(f2), dim, n, batch, 32, BLOCK_N / 2);
+        ok = ok && make_map_3d(&m_b, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<float*>(f2), dim, n, batch, 32, BLOCK_N);
         if (!ok) return MACVO_E_DRIVER;
-        return launch_main<2>(m_a, m_a, m_b, m_b, corr, batch, n, dim, clusters, st);
+        return launch_main<2>(m_a, m_a, m_b, m_b, corr, batch, n, dim, ctas, st);
     }
     if (!workspace || workspace_bytes < macvo_corr_tc_workspace_bytes(batch, dim, n, passes)) return MACVO_E_WORKSPACE;
     if (reinterpret_cast<uintptr_t>(workspace) & 1023) return MACVO_E_ARG;
@@ -495,37 +272,24 @@ int macvo_corr_build_tc(const float* f1, const float* f2, float* corr, int batch
     __half* b_lo = passes == 3 ? reinterpret_cast<__half*>(ws + 3 * ob) : nullptr;
 
     // one launch splits both feature maps: blockIdx.z in [0, batch) -> f1, [batch, 2 batch) -> f2
-    dim3 pgrid(ceil_div(n, 32), ceil_div(dim, 64), 2 * batch);
-    static const int s_dbg_host = [] { const char* e = getenv("MACVO_B200_CORR_DEBUG"); return e ? atoi(e) : 0; }();
-    if (!(s_dbg_host & 16)) {                       // profiling aid (bit 16): reuse the operands of the previous call
-        if (kmajor) {
-            const long long quads = (long long)batch * n * dim / 4;
-            dim3 kgrid((unsigned)((quads + 256 * SPLIT_ILP - 1) / (256 * SPLIT_ILP)), 2);
-            split_kmajor_kernel<<<kgrid, 256, 0, st>>>(f1, f2, a_hi, a_lo, b_hi, b_lo, quads, passes == 3 ? SPLIT_SCALE : 1.f);
-        } else {
-            split_transpose_kernel<<<pgrid, 256, 0, st>>>(f1, f2, a_hi, a_lo, b_hi, b_lo, batch, dim, n,
-                                                          passes == 3 ? SPLIT_SCALE : 1.f);
-        }
-        MACVO_LAUNCH_CHECK();
+    if (kmajor) {
+        const long long quads = (long long)batch * n * dim / 4;
+        dim3 kgrid((unsigned)((quads + 256 * SPLIT_ILP - 1) / (256 * SPLIT_ILP)), 2);
+        split_kmajor_kernel<<<kgrid, 256, 0, st>>>(f1, f2, a_hi, a_lo, b_hi, b_lo, quads, passes == 3 ? SPLIT_SCALE : 1.f);
+    } else {
+        dim3 pgrid(ceil_div(n, 32), ceil_div(dim, 64), 2 * batch);
+        split_transpose_kernel<<<pgrid, 256, 0, st>>>(f1, f2, a_hi, a_lo, b_hi, b_lo, batch, dim, n,
+                                                      passes == 3 ? SPLIT_SCALE : 1.f);
     }
+    MACVO_LAUNCH_CHECK();
 
     CUtensorMap m_a_hi, m_a_lo, m_b_hi, m_b_lo;
-    float* m_out = corr;
     bool ok = make_map_3d(&m_a_hi, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, a_hi, dim, n, batch, BLOCK_K, BLOCK_M);
-    ok = ok && make_map_3d(&m_b_hi, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, b_hi, dim, n, batch, BLOCK_K, BLOCK_N / 2);
+    ok = ok && make_map_3d(&m_b_hi, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, b_hi, dim, n, batch, BLOCK_K, BLOCK_N);
     ok = ok && make_map_3d(&m_a_lo, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, passes == 3 ? a_lo : a_hi, dim, n, batch, BLOCK_K, BLOCK_M);
-    ok = ok && make_map_3d(&m_b_lo, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, passes == 3 ? b_lo : b_hi, dim, n, batch, BLOCK_K, BLOCK_N / 2);
+    ok = ok && make_map_3d(&m_b_lo, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, passes == 3 ? b_lo : b_hi, dim, n, batch, BLOCK_K, BLOCK_N);
     if (!ok) return MACVO_E_DRIVER;
 
-    return passes == 3 ? launch_main<3>(m_a_hi, m_a_lo, m_b_hi, m_b_lo, m_out, batch, n, dim, clusters, st)
-                       : launch_main<1>(m_a_hi, m_a_lo, m_b_hi, m_b_lo, m_out, batch, n, dim, clusters, st);
-}
-
-// profiling aid: copy the last event trace (dbg bit 3) to host memory; returns the number of u64 written
-extern "C" int macvo_corr_debug_trace(unsigned long long* out, int capacity) {
-    if (!g_trace) return 0;
-    cudaDeviceSynchronize();
-    const int n = 2 * 4 * 512 * 2;
-    for (int i = 0; i < n && i < capacity; ++i) out[i] = g_trace[i];
-    return n < capacity ? n : capacity;
+    return passes == 3 ? launch_main<3>(m_a_hi, m_a_lo, m_b_hi, m_b_lo, corr, batch, n, dim, ctas, st)
+                       : launch_main<1>(m_a_hi, m_a_lo, m_b_hi, m_b_lo, corr, batch, n, dim, ctas, st);
 }

@@ -23,7 +23,7 @@
 namespace {
 
 // TP pixels per CTA (template parameter: 64 or 72 — the host picks the one that needs fewer waves of one-CTA-per-SM blocks:
-// 9600 pixels are 150 tiles of 64 = TWO waves on 148 SMs, but 134 tiles of 72 = one), LD = TP + 4 row stride of the
+// e.g. 9000 pixels on 132 SMs: 141 tiles of 64 = TWO waves, 125 tiles of 72 = one), LD = TP + 4 row stride of the
 // [channel][pixel] activation buffers (16-B aligned rows), 4 threads per pixel.
 constexpr int C = 64, CF = 81, OUTC = 160;
 // weight blob (floats): transposed matrices [K][64], then 10 vectors of 64, then 16 frequencies
@@ -307,7 +307,7 @@ extern "C" int macvo_decoder_token(const float* cost_forward, const float* coord
                                    const float* weight_blob, float* out, int batch, int n1, float eps, void* stream) {
     if (!cost_forward || !coords || !key || !value || !weight_blob || !out || batch <= 0 || n1 <= 0) return MACVO_E_ARG;
     const long long pixels = (long long)batch * n1;
-    int dev = 0, sms = 148;
+    int dev = 0, sms = 132;
     MACVO_CUDA_TRY(cudaGetDevice(&dev));
     MACVO_CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
     // one CTA per SM: cost ~ waves x pixels-per-tile
@@ -317,14 +317,14 @@ extern "C" int macvo_decoder_token(const float* cost_forward, const float* coord
                                : launch_token<64>(cost_forward, coords, key, value, weight_blob, out, pixels, n1, eps, st);
 }
 
-/* same, writing fp16 layout-U rows (rows, 192): channels [0,160) = [g | cost_forward | 0], the tcgen05 motion encoder's input */
+/* same, writing fp16 layout-U rows (rows, 192): channels [0,160) = [g | cost_forward | 0], the tensor-core motion encoder's input */
 extern "C" int macvo_decoder_token_rows(const float* cost_forward, const float* coords, const float* key, const float* value,
                                         const float* weight_blob, void* out16_rows, int batch, int height, int width, float eps,
                                         void* stream) {
     if (!cost_forward || !coords || !key || !value || !weight_blob || !out16_rows || batch <= 0 || height <= 0 || width <= 0) return MACVO_E_ARG;
     const int n1 = height * width;
     const long long pixels = (long long)batch * n1;
-    int dev = 0, sms = 148;
+    int dev = 0, sms = 132;
     MACVO_CUDA_TRY(cudaGetDevice(&dev));
     MACVO_CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
     auto cost = [&](int tp) { const long long tiles = (pixels + tp - 1) / tp; return ((tiles + sms - 1) / sms) * tp; };

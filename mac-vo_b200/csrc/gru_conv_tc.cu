@@ -1,4 +1,4 @@
-// (f2) SepConvGRU on the 5th-generation tensor cores: the 1x5 / 5x1 gate convolutions of the decoder's two recurrent units
+// (f2) SepConvGRU on the Hopper tensor cores (wgmma): the 1x5 / 5x1 gate convolutions of the decoder's two recurrent units
 // (flow + covariance) as implicit GEMMs with the gate math in the epilogue. Replaces, per refinement iteration and pass,
 //   zr = conv(cat[h, x]) ; z, r = sigmoid(zr) ; q = tanh(conv(cat[r*h, x])) ; h = (1-z) h + z q
 // (Module/Network/FlowFormer/core/gru.py:22-43, update blocks covhead.py:95-131) — 8 cuDNN convolutions + 8 glue launches per
@@ -6,20 +6,17 @@
 //
 // GEMM view of one stage: rows = pixels (M), columns = output channels (N = 256 for z|r, 128 for q), K = 5 taps x 512
 // channels. Operands are fp16 (11-bit significand >= TF32's 10; the recurrent state itself stays fp32 in `h_master`, only
-// the convolution INPUTS are rounded, like TF32 does on the fly), accumulation fp32 in TMEM.
+// the convolution INPUTS are rounded, like TF32 does on the fly), accumulation fp32 in registers.
 //
 // Layout (csrc/rows_layout.cuh): each pass sees the image as independent LINES along the convolution axis (rows of layout U
 // for 1x5, columns = layout V for 5x1), every line with 2 zero pixels of padding at both ends. A tile is 128
-// consecutive padded pixels; tap t of output pixel p reads pixel p + t - 2. The five tap views of one tile overlap almost
-// entirely, so the A tile (136 rows: pixels p0 - 2 .. p0 + 133, SWIZZLE_128B) is loaded ONCE per 64-channel block and reused
-// by all 5 taps: tap t multiplies rows [t, t + 128), i.e. the UMMA descriptor start advanced by t x 128 B. The 128-byte
-// swizzle is a function of the shared-memory ADDRESS, so a start that is not aligned to the 1024-byte swizzle atom addresses
-// the shifted rows correctly with base_offset 0 (measured: profiles/r02_umma_descriptor_shift_probe.log).
+// consecutive padded pixels; tap t of output pixel p reads pixel p + t - 2, so the A operand of (channel block, tap t) is the
+// 128 rows starting t rows after the tile's first halo pixel, loaded by TMA into its own swizzle-aligned ring slot together
+// with the tap's weight rows.
 // The x part of the input (384 of the 512 channels: context | motion features | aggregated motion) is identical for both
 // units and both stages: it lives in one buffer per layout; the h / r*h part is a separate 128-channel buffer per unit.
 //
-// CTA pairs (cta_group::2): M = 256 per pair, each CTA stages its own A tile and HALF of the weight columns of every
-// (channel block, tap) step; warp 0 = TMA producer, warp 1 = MMA issuer (leader CTA), warps 2..9 = epilogue.
+// One CTA per (unit, 128-pixel tile): warps 0..7 = two consumer warpgroups (m64nNk16 wgmma), warp 8 = TMA producer.
 #include "tc_common.cuh"
 #include "rows_layout.cuh"
 #include <cuda_fp16.h>
@@ -27,17 +24,15 @@
 namespace {
 
 constexpr int HID = 128, XCH = 384, CIN = HID + XCH, TAPS = 5;
-constexpr int TILE_M = macvo_rows::TILE_M, BLOCK_K = 64, UMMA_K = 16, KBLOCKS = CIN / BLOCK_K;     // 8 channel blocks: 2 from h, 6 from x
-constexpr int A_ROWS = 136, A_BYTES = A_ROWS * 128;                                  // 17 KB (TILE_M + 4 halo pixels, rounded to 8 rows)
-constexpr int A_SLOTS = 3;
+constexpr int TILE_M = macvo_rows::TILE_M, BLOCK_K = 64, KBLOCKS = CIN / BLOCK_K;     // 8 channel blocks: 2 from h, 6 from x
+constexpr int A_BYTES = TILE_M * 128;                                                // 16 KB
 constexpr int GUARD = macvo_rows::GUARD;                                             // leading zero rows of every operand buffer
-constexpr int EPI_WARPS = 8;
-constexpr int THREADS = 32 * (2 + EPI_WARPS);
 
 template <int N> struct Cfg {
-    static constexpr int B_BYTES = (N / 2) * 128;                                    // this CTA's half of the weight columns, one (kb, tap) step
-    static constexpr int B_SLOTS = N == 256 ? 8 : 12;
-    static constexpr int SMEM = A_SLOTS * A_BYTES + B_SLOTS * B_BYTES + 512 + 1024;
+    static constexpr int SLOT_BYTES = A_BYTES + N * 128;                             // A rows of one tap + its N weight rows
+    static constexpr int SLOTS = N == 256 ? 4 : 6;
+    static constexpr int SMEM = SLOTS * SLOT_BYTES + 512 + 1024;
+    static_assert(SLOTS * SLOT_BYTES >= TILE_M * N * 4, "the epilogue stages the accumulators in the operand ring");
 };
 
 // MUFU-based gate functions (ex2 + rcp): absolute error ~1e-7, far below the fp16 rounding of the convolution operands
@@ -53,14 +48,14 @@ struct Unit {                    // one recurrent unit (flow / covariance)
 struct Geometry {
     int batch, height, width, vertical;
     int lines, len, lp;          // lines of `len` pixels, padded pitch lp = len + 4
-    int m_pad, pairs;            // padded pixels, CTA pairs per unit
-    unsigned long long* trace;   // profiling aid (NULL in production): globaltimer events of cluster 0's leader, [role][event]
+    int m_pad, tiles;            // padded pixels, 128-pixel tiles per unit
+    unsigned long long* trace;   // profiling aid (NULL in production): globaltimer events of the first CTA, [role][event]
     Timeline tl;                 // profiling aid: in-stream timeline shared with csrc/conv_tc.cu
 };
 
 // STAGE 0: N = 256 (z | r)   STAGE 1: N = 128 (q, then the blend)
 template <int STAGE>
-__global__ void __launch_bounds__(THREADS, 1)
+__global__ void __launch_bounds__(TC_THREADS, 1)
 gru_conv_tc_kernel(const __grid_constant__ CUtensorMap map_h0, const __grid_constant__ CUtensorMap map_h1,
                    const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_w0,
                    const __grid_constant__ CUtensorMap map_w1, Unit u0, Unit u1, Geometry g) {
@@ -68,19 +63,10 @@ gru_conv_tc_kernel(const __grid_constant__ CUtensorMap map_h0, const __grid_cons
     using C = Cfg<N>;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    uint8_t* smem_b = smem + A_SLOTS * A_BYTES;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem_b + C::B_SLOTS * C::B_BYTES);
-    const uint32_t bar_afull = smem_u32(bars), bar_aempty = bar_afull + 8 * A_SLOTS;
-    const uint32_t bar_bfull = bar_aempty + 8 * A_SLOTS, bar_bempty = bar_bfull + 8 * C::B_SLOTS;
-    const uint32_t bar_tfull = bar_bempty + 8 * C::B_SLOTS;
-    uint32_t* tmem_base_slot = reinterpret_cast<uint32_t*>(bars + 2 * A_SLOTS + 2 * C::B_SLOTS + 1);
+    const uint32_t bar_full = smem_u32(smem + C::SLOTS * C::SLOT_BYTES), bar_empty = bar_full + 8 * C::SLOTS;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t rank = cluster_ctarank();
-    const bool leader = rank == 0;
-    const int cluster_id = blockIdx.x >> 1;
-    const int unit = cluster_id / g.pairs, pair = cluster_id - unit * g.pairs;
-    const int tile = 2 * pair + (int)rank;                      // this CTA's 128 padded pixels
+    const int unit = blockIdx.x / g.tiles, tile = blockIdx.x - unit * g.tiles;   // this CTA's 128 padded pixels
     const Unit u = unit == 0 ? u0 : u1;
     const CUtensorMap* map_h = unit == 0 ? &map_h0 : &map_h1;
     const CUtensorMap* map_w = unit == 0 ? &map_w0 : &map_w1;
@@ -93,192 +79,144 @@ gru_conv_tc_kernel(const __grid_constant__ CUtensorMap map_h0, const __grid_cons
             g.trace[role * 64 + tr_n++] = t;
         }
     };
-    if (warp == 2 && lane == 0) TR(2);
+    if (warp == 0 && lane == 0) TR(2);
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < A_SLOTS; ++s) { mbar_init(bar_afull + 8 * s, 1); mbar_init(bar_aempty + 8 * s, 1); }
-        for (int s = 0; s < C::B_SLOTS; ++s) { mbar_init(bar_bfull + 8 * s, 1); mbar_init(bar_bempty + 8 * s, 1); }
-        mbar_init(bar_tfull, 1);
+        for (int s = 0; s < C::SLOTS; ++s) { mbar_init(bar_full + 8 * s, 1); mbar_init(bar_empty + 8 * s, 2); }
         fence_barrier_init();
         prefetch_tmap(map_h); prefetch_tmap(&map_x); prefetch_tmap(map_w);
     }
-    if (warp == 1) tmem_alloc(smem_u32(tmem_base_slot), N);
-    tc_fence_before();
     __syncthreads();
-    cluster_sync_all();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_base_slot;
     // Programmatic dependent launch: the next stage may start as soon as every CTA of this one got here. Its weights and the x
     // part of its input (6 of the 8 channel blocks) do not depend on this stage, so the K loop runs the x blocks FIRST and only
     // the h / r*h blocks (and the epilogue's reads of h_master / z) wait for the previous stage (`griddepcontrol.wait`).
     asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-    if (warp == 2 && lane == 0) TR(2);
 
-    if (warp == 0) {
-        // ===================== TMA producer (both CTAs; completion lands on the leader's barriers) =====================
+    if (warp == TC_PRODUCER_WARP) {
+        // ===================== TMA producer =====================
         if (elect_one()) {
-            int aslot = 0, bslot = 0; uint32_t aphase = 0, bphase = 0;
+            int slot = 0; uint32_t phase = 0;
             TR(0);
             for (int it = 0; it < KBLOCKS; ++it) {
                 const int kb = (it + HID / BLOCK_K) % KBLOCKS;                 // 2, 3, ..., 7, 0, 1
                 if (kb == 0) asm volatile("griddepcontrol.wait;" ::: "memory");
-                mbar_wait(bar_aempty + 8 * aslot, aphase ^ 1);
-                const uint32_t afull = bar_afull + 8 * aslot;
-                if (leader) mbar_expect_tx(afull, 2 * A_BYTES);
-                if (kb < HID / BLOCK_K) tma_load_2d_2cta(smem_u32(smem + aslot * A_BYTES), map_h, afull, kb * BLOCK_K, tile * TILE_M);
-                else tma_load_2d_2cta(smem_u32(smem + aslot * A_BYTES), &map_x, afull, kb * BLOCK_K - HID, tile * TILE_M);
-                if (++aslot == A_SLOTS) { aslot = 0; aphase ^= 1; }
                 for (int t = 0; t < TAPS; ++t) {
-                    mbar_wait(bar_bempty + 8 * bslot, bphase ^ 1);
+                    mbar_wait(bar_empty + 8 * slot, phase ^ 1);
                     TR(0);
-                    const uint32_t bfull = bar_bfull + 8 * bslot;
-                    if (leader) mbar_expect_tx(bfull, 2 * C::B_BYTES);
-                    tma_load_2d_2cta(smem_u32(smem_b + bslot * C::B_BYTES), map_w, bfull, t * CIN + kb * BLOCK_K, (int)rank * (N / 2));
-                    if (++bslot == C::B_SLOTS) { bslot = 0; bphase ^= 1; }
+                    const uint32_t full = bar_full + 8 * slot, sa = smem_u32(smem + slot * C::SLOT_BYTES);
+                    mbar_expect_tx(full, C::SLOT_BYTES);
+                    if (kb < HID / BLOCK_K) tma_load_2d(sa, map_h, full, kb * BLOCK_K, tile * TILE_M + t);
+                    else tma_load_2d(sa, &map_x, full, kb * BLOCK_K - HID, tile * TILE_M + t);
+                    tma_load_2d(sa + A_BYTES, map_w, full, t * CIN + kb * BLOCK_K, 0);
+                    if (++slot == C::SLOTS) { slot = 0; phase ^= 1; }
                 }
             }
         }
-    } else if (warp == 1) {
-        // ===================== MMA issuer: leader CTA, cta_group::2, both operands from shared memory =====================
-        if (leader) {
-            constexpr uint32_t idesc = make_idesc_f16(2 * TILE_M, N);
-            int aslot = 0, bslot = 0; uint32_t aphase = 0, bphase = 0;
-            for (int kb = 0; kb < KBLOCKS; ++kb) {
-                mbar_wait(bar_afull + 8 * aslot, aphase);
-                const uint32_t sa = smem_u32(smem + aslot * A_BYTES);
-                for (int t = 0; t < TAPS; ++t) {
-                    mbar_wait(bar_bfull + 8 * bslot, bphase);
-                    tc_fence_after();
-                    if (lane == 0) TR(1);
-                    if (elect_one()) {
-                        const uint64_t da = make_kmajor_sw128_desc(sa + t * 128);        // tap t = rows [t, t + 128)
-                        const uint64_t db = make_kmajor_sw128_desc(smem_u32(smem_b + bslot * C::B_BYTES));
+        return;
+    }
+
+    // ===================== consumers: MMAs (one group in flight) =====================
+    const int wg = warp >> 2;
+    float acc[N / 2];
+    {
+        int slot = 0, prev = 0; uint32_t phase = 0;
+        for (int s = 0; s < KBLOCKS * TAPS; ++s) {
+            mbar_wait(bar_full + 8 * slot, phase);
+            if (warp == 0 && lane == 0) TR(1);
+            const uint32_t sa = smem_u32(smem + slot * C::SLOT_BYTES);
+            const uint64_t da = make_kmajor_sw128_desc(sa + wg * 64 * 128), db = make_kmajor_sw128_desc(sa + A_BYTES);
+            wgmma_fence();
 #pragma unroll
-                        for (int k = 0; k < BLOCK_K / UMMA_K; ++k)
-                            umma_f16_ss2(tmem_base, da + 2 * k, db + 2 * k, idesc, (kb | t | k) != 0);   // `kb` here is the loop count
-                        umma_commit_mc(bar_bempty + 8 * bslot, 3);
-                        if (t == TAPS - 1) umma_commit_mc(bar_aempty + 8 * aslot, 3);
-                        if (t == TAPS - 1 && kb == KBLOCKS - 1) umma_commit_mc(bar_tfull, 3);
-                    }
-                    __syncwarp();
-                    if (++bslot == C::B_SLOTS) { bslot = 0; bphase ^= 1; }
-                }
-                if (++aslot == A_SLOTS) { aslot = 0; aphase ^= 1; }
-            }
+            for (int k = 0; k < BLOCK_K / 16; ++k) Wgmma<N>::f16(acc, da + 2 * k, db + 2 * k, (s | k) != 0);
+            wgmma_commit();
+            wgmma_wait<1>();
+            if (s > 0 && (threadIdx.x & 127) == 0) mbar_arrive(bar_empty + 8 * prev);
+            prev = slot;
+            if (++slot == C::SLOTS) { slot = 0; phase ^= 1; }
         }
-    } else {
-        // ===================== epilogue: TMEM -> registers -> smem transpose -> gate math -> coalesced global ==============
-        // warp w reads TMEM lanes [32 (w & 3), +32); the two warps of a lane quarter split the columns. tcgen05.ld hands every
-        // lane one accumulator ROW; touching global memory that way costs 32 cache lines per warp instruction (an event trace
-        // of the first version showed the epilogue taking 12 us against 11 us of MMAs), so each quarter transposes through the
-        // (now idle) operand ring: rows of N floats, 16-byte chunks XOR-swizzled by the row -> conflict-free both ways, and
-        // global memory is then accessed one full pixel row (512 B) per warp instruction.
-        const int quarter = warp & 3, half = (warp - 2) >> 2;
-        const int m = quarter * 32 + lane;
-        const int pp = tile * TILE_M + m;                                 // padded pixel of this accumulator row
-        const int line = pp / g.lp, pos = pp - line * g.lp - 2;
-        int dense = 0, other = 0;                                         // dense pixel index | operand row in the other pass's layout
-        bool valid = pp < g.m_pad && pos >= 0 && pos < g.len;
+        wgmma_wait<0>();
+        fence_acc(acc);
+    }
+
+    // ===================== epilogue: accumulators -> smem transpose -> gate math -> coalesced global ==============
+    // The accumulator fragment holds scattered (row, column pair) elements; each warpgroup stages its 64 rows through the (now idle)
+    // operand ring as rows of N floats, 16-byte chunks XOR-swizzled by the row -> conflict-free reads, and global memory is
+    // then accessed one full pixel row (512 B) per warp instruction. Warp (quarter, half) owns rows [32 quarter, +32).
+    consumers_sync();                                                     // every MMA of both warpgroups read its operands
+    stage_acc_rows<N>(smem_u32(smem) + wg * 64 * (N * 4), N * 4, acc, 0);
+    const int quarter = warp & 3, half = warp >> 2;
+    const int m = quarter * 32 + lane;
+    const int pp = tile * TILE_M + m;                                 // padded pixel of this accumulator row
+    const int line = pp / g.lp, pos = pp - line * g.lp - 2;
+    int dense = 0, other = 0;                                         // dense pixel index | operand row in the other pass's layout
+    bool valid = pp < g.m_pad && pos >= 0 && pos < g.len;
+    if (valid) {
+        int b, y, x;
+        if (!g.vertical) { b = line / (g.height + 4); y = line - b * (g.height + 4) - 2; x = pos; valid = y >= 0 && y < g.height; }
+        else { b = line / g.width; x = line - b * g.width; y = pos; }
         if (valid) {
-            int b, y, x;
-            if (!g.vertical) { b = line / (g.height + 4); y = line - b * (g.height + 4) - 2; x = pos; valid = y >= 0 && y < g.height; }
-            else { b = line / g.width; x = line - b * g.width; y = pos; }
-            if (valid) {
-                dense = (b * g.height + y) * g.width + x;
-                other = (int)(!g.vertical ? macvo_rows::vrow(b, y, x, g.height, g.width) : macvo_rows::urow(b, y, x, g.height, g.width));
-            }
+            dense = (b * g.height + y) * g.width + x;
+            other = (int)(!g.vertical ? macvo_rows::vrow(b, y, x, g.height, g.width) : macvo_rows::urow(b, y, x, g.height, g.width));
         }
-        const uint32_t vmask = __ballot_sync(0xffffffffu, valid);
-        const uint32_t stage_q = smem_u32(smem) + quarter * (32 * N * 4);   // this quarter's 32 rows x N fp32
-        // The state rows this warp will need (h for r*h | h and z for the blend) depend only on the PREVIOUS stage: fetch them into
-        // registers now, while the MMAs of this stage are still running (a first version loaded them row by row inside the loop
-        // below: 32 dependent L2 round trips per warp, 13 us on the event trace).
-        asm volatile("griddepcontrol.wait;" ::: "memory");
-        constexpr int ROWS = STAGE == 0 ? 32 : 16;                        // rows finished by this warp
-        const int row0 = STAGE == 0 ? 0 : half * 16;
-        float4 hh[ROWS], zz[STAGE == 0 ? 1 : ROWS];
-        if (STAGE == 1 || half == 1) {
+    }
+    const uint32_t vmask = __ballot_sync(0xffffffffu, valid);
+    const uint32_t stage_q = smem_u32(smem) + quarter * (32 * N * 4);   // this quarter's 32 rows x N fp32
+    // the state rows this warp needs (h for r*h | h and z for the blend) were written by the PREVIOUS stage
+    asm volatile("griddepcontrol.wait;" ::: "memory");
+    constexpr int ROWS = STAGE == 0 ? 32 : 16;                        // rows finished by this warp
+    const int row0 = STAGE == 0 ? 0 : half * 16;
+    float4 hh[ROWS], zz[STAGE == 0 ? 1 : ROWS];
+    if (STAGE == 1 || half == 1) {
 #pragma unroll
-            for (int i = 0; i < ROWS; ++i) {
-                const long long d = __shfl_sync(0xffffffffu, dense, row0 + i);          // invalid rows carry 0: a harmless read
-                hh[i] = *reinterpret_cast<const float4*>(u.h_master + d * HID + 4 * lane);
-                if (STAGE == 1) zz[i] = *reinterpret_cast<const float4*>(u.z + d * HID + 4 * lane);
-            }
+        for (int i = 0; i < ROWS; ++i) {
+            const long long d = __shfl_sync(0xffffffffu, dense, row0 + i);          // invalid rows carry 0: a harmless read
+            hh[i] = *reinterpret_cast<const float4*>(u.h_master + d * HID + 4 * lane);
+            if (STAGE == 1) zz[i] = *reinterpret_cast<const float4*>(u.z + d * HID + 4 * lane);
         }
-        if (warp == 2 && lane == 0) TR(2);
-        mbar_wait(bar_tfull, 0);
-        tc_fence_after();
-        if (warp == 2 && lane == 0) TR(2);
-        const uint32_t trow = tmem_base + ((uint32_t)(quarter * 32) << 16);
-        constexpr int COLS = N / 2;                                       // columns drained by this warp
-        {
-            uint32_t r[32];
-#pragma unroll 1
-            for (int c = 0; c < COLS / 32; ++c) {
-                tmem_ld_32x32b_x32(trow + half * COLS + c * 32, r);
-                tmem_ld_wait();
+    }
+    consumers_sync();                                                     // all rows staged
+    if (warp == 0 && lane == 0) TR(2);
+    if (STAGE == 0) {
+        // half 0: z columns [0, 128) -> z buffer      half 1: r columns [128, 256) -> r * h operand rows (this layout)
+        const float4 bb = __ldg(reinterpret_cast<const float4*>(u.bias + half * 128 + 4 * lane));
 #pragma unroll
-                for (int e = 0; e < 8; ++e) {
-                    const int c16 = (half * COLS + c * 32) / 4 + e;
-                    sts128(stage_q + lane * (N * 4) + ((c16 ^ (lane & 7)) << 4),
-                           make_float4(__uint_as_float(r[4 * e]), __uint_as_float(r[4 * e + 1]), __uint_as_float(r[4 * e + 2]),
-                                       __uint_as_float(r[4 * e + 3])));
-                }
-            }
-        }
-        if (STAGE == 0) {
-            // half 0: z columns [0, 128) -> z buffer      half 1: r columns [128, 256) -> r * h operand rows (this layout)
-            __syncwarp();                                                  // each warp reads back only what it wrote
-            const float4 bb = __ldg(reinterpret_cast<const float4*>(u.bias + half * 128 + 4 * lane));
-#pragma unroll
-            for (int rr = 0; rr < 32; ++rr) {
-                const long long d = __shfl_sync(0xffffffffu, dense, rr);
-                if (!((vmask >> rr) & 1u)) continue;
-                const int c16 = half * 32 + lane;
-                const float4 v = lds128(stage_q + rr * (N * 4) + ((c16 ^ (rr & 7)) << 4));
-                float4 o;
-                o.x = sigmoid_fast(v.x + bb.x); o.y = sigmoid_fast(v.y + bb.y); o.z = sigmoid_fast(v.z + bb.z); o.w = sigmoid_fast(v.w + bb.w);
-                if (half == 0) {
-                    *reinterpret_cast<float4*>(u.z + d * HID + 4 * lane) = o;
-                } else {
-                    __half2 h2[2] = {__floats2half2_rn(o.x * hh[rr].x, o.y * hh[rr].y), __floats2half2_rn(o.z * hh[rr].z, o.w * hh[rr].w)};
-                    const long long orow = (long long)GUARD + tile * TILE_M + quarter * 32 + rr;
-                    *reinterpret_cast<uint2*>(u.out + orow * HID + 4 * lane) = *reinterpret_cast<uint2*>(h2);
-                }
-            }
-        } else {
-            // h <- (1 - z) h + z tanh(q + bias)   (same association as gru.py:33,41); warp `half` finishes rows [16 half, +16)
-            asm volatile("bar.sync %0, 64;" ::"r"(1 + quarter) : "memory");   // both warps of the quarter staged their columns
-            const float4 bb = __ldg(reinterpret_cast<const float4*>(u.bias + 4 * lane));
-#pragma unroll
-            for (int i = 0; i < 16; ++i) {
-                const int rr = row0 + i;
-                const long long d = __shfl_sync(0xffffffffu, dense, rr);
-                const long long orow = __shfl_sync(0xffffffffu, other, rr);
-                if (!((vmask >> rr) & 1u)) continue;
-                const float4 v = lds128(stage_q + rr * (N * 4) + ((lane ^ (rr & 7)) << 4));
-                const float4 h4 = hh[i], z4 = zz[STAGE == 0 ? 0 : i];
-                float4 n;
-                n.x = (1.f - z4.x) * h4.x + z4.x * tanh_fast(v.x + bb.x);
-                n.y = (1.f - z4.y) * h4.y + z4.y * tanh_fast(v.y + bb.y);
-                n.z = (1.f - z4.z) * h4.z + z4.z * tanh_fast(v.z + bb.z);
-                n.w = (1.f - z4.w) * h4.w + z4.w * tanh_fast(v.w + bb.w);
-                *reinterpret_cast<float4*>(u.h_master + d * HID + 4 * lane) = n;
-                __half2 h2[2] = {__floats2half2_rn(n.x, n.y), __floats2half2_rn(n.z, n.w)};
+        for (int rr = 0; rr < 32; ++rr) {
+            const long long d = __shfl_sync(0xffffffffu, dense, rr);
+            if (!((vmask >> rr) & 1u)) continue;
+            const int c16 = half * 32 + lane;
+            const float4 v = lds128(stage_q + rr * (N * 4) + ((c16 ^ (rr & 7)) << 4));
+            float4 o;
+            o.x = sigmoid_fast(v.x + bb.x); o.y = sigmoid_fast(v.y + bb.y); o.z = sigmoid_fast(v.z + bb.z); o.w = sigmoid_fast(v.w + bb.w);
+            if (half == 0) {
+                *reinterpret_cast<float4*>(u.z + d * HID + 4 * lane) = o;
+            } else {
+                __half2 h2[2] = {__floats2half2_rn(o.x * hh[rr].x, o.y * hh[rr].y), __floats2half2_rn(o.z * hh[rr].z, o.w * hh[rr].w)};
+                const long long orow = (long long)GUARD + tile * TILE_M + quarter * 32 + rr;
                 *reinterpret_cast<uint2*>(u.out + orow * HID + 4 * lane) = *reinterpret_cast<uint2*>(h2);
             }
         }
+    } else {
+        // h <- (1 - z) h + z tanh(q + bias)   (same association as gru.py:33,41); warp `half` finishes rows [16 half, +16)
+        const float4 bb = __ldg(reinterpret_cast<const float4*>(u.bias + 4 * lane));
+#pragma unroll
+        for (int i = 0; i < 16; ++i) {
+            const int rr = row0 + i;
+            const long long d = __shfl_sync(0xffffffffu, dense, rr);
+            const long long orow = __shfl_sync(0xffffffffu, other, rr);
+            if (!((vmask >> rr) & 1u)) continue;
+            const float4 v = lds128(stage_q + rr * (N * 4) + ((lane ^ (rr & 7)) << 4));
+            const float4 h4 = hh[i], z4 = zz[STAGE == 0 ? 0 : i];
+            float4 n;
+            n.x = (1.f - z4.x) * h4.x + z4.x * tanh_fast(v.x + bb.x);
+            n.y = (1.f - z4.y) * h4.y + z4.y * tanh_fast(v.y + bb.y);
+            n.z = (1.f - z4.z) * h4.z + z4.z * tanh_fast(v.z + bb.z);
+            n.w = (1.f - z4.w) * h4.w + z4.w * tanh_fast(v.w + bb.w);
+            *reinterpret_cast<float4*>(u.h_master + d * HID + 4 * lane) = n;
+            __half2 h2[2] = {__floats2half2_rn(n.x, n.y), __floats2half2_rn(n.z, n.w)};
+            *reinterpret_cast<uint2*>(u.out + orow * HID + 4 * lane) = *reinterpret_cast<uint2*>(h2);
+        }
     }
-
-    if (warp == 2 && lane == 0) TR(2);
-    tc_fence_before();
-    __syncthreads();
-    cluster_sync_relaxed();                   // no CTA exits while its peer may still signal / read its shared memory
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, N);
-    }
-    if (warp == 2 && lane == 0) TR(2);
+    if (warp == 0 && lane == 0) TR(2);
     g.tl.end();
 }
 
@@ -328,17 +266,17 @@ Geometry make_geometry(int batch, int height, int width, int vertical) {
     g.len = vertical ? height : width;
     g.lp = g.len + 4;
     g.m_pad = g.lines * g.lp;
-    g.pairs = (g.m_pad + 2 * TILE_M - 1) / (2 * TILE_M);
+    g.tiles = (g.m_pad + TILE_M - 1) / TILE_M;
     g.trace = nullptr;
     g.tl = Timeline{nullptr, 0, -1};
     return g;
 }
 size_t operand_rows(const Geometry& g) { return (size_t)macvo_rows::alloc_rows(g.batch, g.height, g.width, g.vertical); }
 
-// A operand: (rows, channels) fp16, box = 136 rows x 64 channels starting at the tile's first halo pixel (operand row = padded
-// pixel + GUARD, so the box of tile t starts at row 128 t)
+// A operand: (rows, channels) fp16, box = 128 rows x 64 channels; tap t of tile i starts at row 128 i + t (operand row = padded
+// pixel + GUARD, so that row is padded pixel 128 i + t - 2, the tap's input of the tile's first pixel)
 bool make_map_a(CUtensorMap* map, const void* base, int channels, const Geometry& g) {
-    return make_map_2d(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, base, channels, operand_rows(g), (uint64_t)channels * 2, BLOCK_K, A_ROWS);
+    return make_map_2d(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, base, channels, operand_rows(g), (uint64_t)channels * 2, BLOCK_K, TILE_M);
 }
 
 template <int STAGE>
@@ -350,17 +288,15 @@ int launch_stage(const CUtensorMap* maps, Unit u0, Unit u1, const Geometry& g, i
         configured = true;
     }
     cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(2 * g.pairs * units);
-    cfg.blockDim = dim3(THREADS);
+    cfg.gridDim = dim3(g.tiles * units);
+    cfg.blockDim = dim3(TC_THREADS);
     cfg.dynamicSmemBytes = Cfg<N>::SMEM;
     cfg.stream = stream;
-    cudaLaunchAttribute attrs[2];
-    attrs[0].id = cudaLaunchAttributeClusterDimension;
-    attrs[0].val.clusterDim.x = 2; attrs[0].val.clusterDim.y = 1; attrs[0].val.clusterDim.z = 1;
-    attrs[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attrs[1].val.programmaticStreamSerializationAllowed = 1;
+    cudaLaunchAttribute attrs[1];
+    attrs[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attrs[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attrs;
-    cfg.numAttrs = 2;
+    cfg.numAttrs = 1;
     MACVO_CUDA_TRY(cudaLaunchKernelEx(&cfg, gru_conv_tc_kernel<STAGE>, maps[0], maps[1], maps[2], maps[3], maps[4], u0, u1, g));
     return MACVO_OK;
 }
@@ -369,7 +305,7 @@ int launch_stage(const CUtensorMap* maps, Unit u0, Unit u1, const Geometry& g, i
 
 Timeline macvo_tc_timeline();          // csrc/conv_tc.cu
 static unsigned long long* g_trace = nullptr;
-/* profiling aid (tools/gru_probe.py): device buffer of 3 x 64 u64 that cluster 0's leader fills with globaltimer events */
+/* profiling aid (tools/gru_probe.py): device buffer of 3 x 64 u64 that the first CTA fills with globaltimer events */
 extern "C" void macvo_gru_tc_set_trace(void* buf) { g_trace = static_cast<unsigned long long*>(buf); }
 
 extern "C" size_t macvo_gru_tc_operand_rows(int batch, int height, int width, int vertical) {
@@ -383,7 +319,7 @@ extern "C" int macvo_gru_tc_pack(const float* src, int src_pitch, int channels, 
         src_pitch < channels || src_pitch % 4 || dst_offset + channels > dst_channels)
         return MACVO_E_ARG;
     const long long total = (long long)batch * height * width * (channels / 4);
-    const int blocks = (int)((total + 255) / 256 < 148 * 8 ? (total + 255) / 256 : 148 * 8);
+    const int blocks = (int)((total + 255) / 256 < 132 * 8 ? (total + 255) / 256 : 132 * 8);
     pack_rows_kernel<<<blocks, 256, 0, as_stream(stream)>>>(src, src_pitch, channels, static_cast<__half*>(dst), dst_channels, dst_offset,
                                                             batch, height, width, vertical);
     MACVO_LAUNCH_CHECK();
@@ -394,7 +330,7 @@ extern "C" int macvo_gru_tc_pack_motion(const float* mf, const float* agg, const
                                         int batch, int height, int width, void* stream) {
     if (!mf || !agg || !gamma || !x_rows_h || !x_rows_v || batch <= 0 || height <= 0 || width <= 0) return MACVO_E_ARG;
     const long long total = (long long)batch * height * width * (HID / 4);
-    const int blocks = (int)((total + 255) / 256 < 148 * 8 ? (total + 255) / 256 : 148 * 8);
+    const int blocks = (int)((total + 255) / 256 < 132 * 8 ? (total + 255) / 256 : 132 * 8);
     pack_motion_kernel<<<blocks, 256, 0, as_stream(stream)>>>(mf, agg, gamma, static_cast<__half*>(x_rows_h), static_cast<__half*>(x_rows_v),
                                                               batch, height, width);
     MACVO_LAUNCH_CHECK();
@@ -418,7 +354,7 @@ extern "C" int macvo_gru_tc_stage(int stage, int vertical, int batch, int height
         const int s = i < units ? i : 0;
         if (!make_map_a(&maps[i], h_rows[s], HID, g)) return MACVO_E_UNSUPPORTED;
         if (!make_map_2d(&maps[3 + i], CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, weights[s], (uint64_t)TAPS * CIN, n, (uint64_t)TAPS * CIN * 2,
-                         BLOCK_K, n / 2))
+                         BLOCK_K, n))
             return MACVO_E_UNSUPPORTED;
     }
     if (!make_map_a(&maps[2], x_rows, XCH, g)) return MACVO_E_UNSUPPORTED;

@@ -1,5 +1,5 @@
 // Frontend "next" rows (SURVEY.md §8f-1/2): the memory-bound glue of the FlowFormerCov cost perceiver that
-// cuDNN / ATen run far below HBM speed at these shapes (measured on B200, profiles/r01_probe_attention.log):
+// cuDNN / ATen run far below HBM speed at these shapes (SURVEY.md §8f):
 //
 //   layer_norm          (9600*80, 128) fp32: ATen 1136 us for 786 MB of traffic      -> warp-per-row kernel
 //   patch_embed_conv1   1 -> 16 ch, 6x6 stride 2 over 9600 cost maps: cuDNN 3636 us  -> direct conv, map in smem,
@@ -14,6 +14,10 @@
 #include <math_constants.h>
 
 namespace {
+
+// float2 multiply-add / multiply, one correctly rounded FMA / FMUL per component (sm_90 has no paired FFMA2 instruction)
+__device__ __forceinline__ float2 ffma2_rn(float2 a, float2 b, float2 c) { return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)); }
+__device__ __forceinline__ float2 fmul2_rn(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
 
 // ---- LayerNorm over the last dimension, one warp per row, C = 32 * VPL --------------------------------
 template <int VPL>
@@ -211,8 +215,8 @@ attn_shared_kv_kernel(const float* __restrict__ q, const float* __restrict__ k, 
 #pragma unroll
             for (int c = 0; c < D / 4; ++c) {
                 const float4 kk = kj[c];
-                t = __ffma2_rn(qr[2 * c], make_float2(kk.x, kk.y), t);
-                t = __ffma2_rn(qr[2 * c + 1], make_float2(kk.z, kk.w), t);
+                t = ffma2_rn(qr[2 * c], make_float2(kk.x, kk.y), t);
+                t = ffma2_rn(qr[2 * c + 1], make_float2(kk.z, kk.w), t);
             }
             s[u] = (j0 + u < nk) ? t.x + t.y : -CUDART_INF_F;
         }
@@ -224,7 +228,7 @@ attn_shared_kv_kernel(const float* __restrict__ q, const float* __restrict__ k, 
         l *= corr;
         const float2 c2 = make_float2(corr, corr);
 #pragma unroll
-        for (int c = 0; c < D / 2; ++c) acc[c] = __fmul2_rn(acc[c], c2);
+        for (int c = 0; c < D / 2; ++c) acc[c] = fmul2_rn(acc[c], c2);
 #pragma unroll
         for (int u = 0; u < ATT_CHUNK; ++u) {
             const float p = __expf(s[u] - mn);
@@ -234,8 +238,8 @@ attn_shared_kv_kernel(const float* __restrict__ q, const float* __restrict__ k, 
 #pragma unroll
             for (int c = 0; c < D / 4; ++c) {
                 const float4 vv = vj[c];
-                acc[2 * c] = __ffma2_rn(p2, make_float2(vv.x, vv.y), acc[2 * c]);
-                acc[2 * c + 1] = __ffma2_rn(p2, make_float2(vv.z, vv.w), acc[2 * c + 1]);
+                acc[2 * c] = ffma2_rn(p2, make_float2(vv.x, vv.y), acc[2 * c]);
+                acc[2 * c + 1] = ffma2_rn(p2, make_float2(vv.z, vv.w), acc[2 * c + 1]);
             }
         }
     }
@@ -634,8 +638,8 @@ attn_few_queries_kernel(const float* __restrict__ q, const float* __restrict__ k
             float2 sx = make_float2(0.f, 0.f);
 #pragma unroll
             for (int c = 0; c < FQ_D / 4; ++c) {
-                sx = __ffma2_rn(qr[t][2 * c], make_float2(kk[c].x, kk[c].y), sx);
-                sx = __ffma2_rn(qr[t][2 * c + 1], make_float2(kk[c].z, kk[c].w), sx);
+                sx = ffma2_rn(qr[t][2 * c], make_float2(kk[c].x, kk[c].y), sx);
+                sx = ffma2_rn(qr[t][2 * c + 1], make_float2(kk[c].z, kk[c].w), sx);
             }
             const float s = sx.x + sx.y;
             const float mn = fmaxf(m[t], s);
@@ -645,8 +649,8 @@ attn_few_queries_kernel(const float* __restrict__ q, const float* __restrict__ k
             const float2 c2 = make_float2(corr, corr), p2 = make_float2(p, p);
 #pragma unroll
             for (int c = 0; c < FQ_D / 4; ++c) {
-                acc[t][2 * c] = __ffma2_rn(p2, make_float2(vv[c].x, vv[c].y), __fmul2_rn(acc[t][2 * c], c2));
-                acc[t][2 * c + 1] = __ffma2_rn(p2, make_float2(vv[c].z, vv[c].w), __fmul2_rn(acc[t][2 * c + 1], c2));
+                acc[t][2 * c] = ffma2_rn(p2, make_float2(vv[c].x, vv[c].y), fmul2_rn(acc[t][2 * c], c2));
+                acc[t][2 * c + 1] = ffma2_rn(p2, make_float2(vv[c].z, vv[c].w), fmul2_rn(acc[t][2 * c + 1], c2));
             }
         }
     }

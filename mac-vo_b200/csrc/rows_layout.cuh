@@ -24,7 +24,7 @@ __host__ __device__ inline long long urow(int b, int y, int x, int height, int w
 __host__ __device__ inline long long vrow(int b, int y, int x, int height, int width) {
     return (long long)GUARD + ((long long)b * width + x) * (height + 4) + y + 2;
 }
-// padded pixel count (rows between the guards) and allocation size in rows (tiles of 128, CTA pairs of 256, + guards)
+// padded pixel count (rows between the guards) and allocation size in rows (rounded up to a multiple of 256 rows, + guards)
 __host__ __device__ inline int padded_pixels(int batch, int height, int width, int vertical) {
     return vertical ? batch * width * (height + 4) : batch * (height + 4) * (width + 4);
 }

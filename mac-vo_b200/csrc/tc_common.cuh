@@ -1,12 +1,20 @@
-// tcgen05 / TMEM / TMA / mbarrier PTX wrappers and host-side tensor-map helpers shared by the sm_100a tensor-core kernels
-// (corr_build_tc.cu: correlation volume, CTA pairs; conv_tc.cu: decoder convolutions, single CTAs).
-// Descriptor bit layouts follow the public CUTLASS / CuTe conventions (cute::UMMA::SmemDescriptor / InstrDescriptor).
+// wgmma / TMA / mbarrier PTX wrappers and host-side tensor-map helpers shared by the sm_90a tensor-core kernels
+// (corr_build_tc.cu: correlation volume; conv_tc.cu: decoder convolutions; gru_conv_tc.cu: SepConvGRU gates).
+//
+// All three share one CTA shape: warps 0..7 are two consumer warpgroups that issue wgmma (each owns 64 rows of the 128-row
+// tile, fp32 accumulators in registers), warp 8 is the TMA producer feeding an mbarrier-guarded shared-memory ring.
+// Descriptor bit layouts follow the PTX ISA (wgmma matrix descriptor) and the public CUTLASS / CuTe GmmaDescriptor.
 #pragma once
 #include "common.cuh"
+#include "wgmma_ops.cuh"
 #include <cuda.h>
 #include <mutex>
 
 namespace {
+
+constexpr int TC_CONSUMER_THREADS = 256;                   // two warpgroups
+constexpr int TC_THREADS = TC_CONSUMER_THREADS + 32;       // + the producer warp
+constexpr int TC_PRODUCER_WARP = 8;
 
 // ---- PTX wrappers ---------------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -16,6 +24,9 @@ __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
 }
 __device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
 __device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
     uint32_t ok;
@@ -43,163 +54,68 @@ __device__ __forceinline__ bool elect_one() {
         : "=r"(pred));
     return pred != 0;
 }
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-    return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// execution-only rendezvous of the cluster (no memory ordering): used before exit, where the default .release arrive would first
-// wait for every in-flight global store of the epilogue to be acknowledged (2-4 us on the event traces of the decoder kernels)
-__device__ __forceinline__ void cluster_sync_relaxed() {
-    asm volatile("barrier.cluster.arrive.relaxed.aligned;\n\tbarrier.cluster.wait.aligned;" ::: "memory");
-}
-constexpr uint32_t PEER_BIT_MASK = 0xFEFFFFFFu;    // shared-window address with the CTA-pair rank bit cleared -> CTA 0
-// 2-CTA TMA load: data lands in THIS CTA's smem, the complete_tx goes to the LEADER CTA's mbarrier
-__device__ __forceinline__ void tma_load_3d_2cta(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, int c2) {
+__device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
+// the two consumer warpgroups only (the producer warp never joins): named barrier 1
+__device__ __forceinline__ void consumers_sync() { asm volatile("bar.sync 1, %0;" ::"n"(TC_CONSUMER_THREADS) : "memory"); }
+
+__device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1) {
     asm volatile(
-        "cp.async.bulk.tensor.3d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-        ::"r"(dst), "l"(map), "r"(bar & PEER_BIT_MASK), "r"(c0), "r"(c1), "r"(c2) : "memory");
+        "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
+        ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1) : "memory");
 }
-// arrive on the barrier at the same offset in CTA `rank` of the cluster. RELAXED: the arrive only hands a TMEM accumulator
-// back (its reads are complete: tcgen05.wait::ld + tcgen05.fence::before_thread_sync); it publishes no generic-proxy memory.
-// With .release the arrive waited for the warp's in-flight global stores of the previous half tile — ncu attributed 24 % of
-// all warp stall samples of v7 to this one instruction (membar + mio), on the critical path of the next tile's MMAs.
-__device__ __forceinline__ void mbar_arrive_remote(uint32_t bar, uint32_t rank) {
+__device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, int c2) {
     asm volatile(
-        "{\n\t.reg .b32 ra;\n\t"
-        "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
-        "mbarrier.arrive.relaxed.cluster.shared::cluster.b64 _, [ra];\n\t}"
-        ::"r"(bar), "r"(rank) : "memory");
+        "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
+        ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1), "r"(c2) : "memory");
 }
-// explicit shared-space vector accesses for the epilogue transpose: through the generic `uint8_t*` the compiler emitted
-// LD.E / ST.E (generic address path, long-scoreboard latency) — ncu showed the epilogue warps waiting on exactly those
-__device__ __forceinline__ void sts128(uint32_t addr, float4 v) {
-    asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w) : "memory");
+__device__ __forceinline__ void prefetch_tmap(const CUtensorMap* map) {
+    asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
+}
+
+// explicit shared-space vector accesses for the epilogue transposes (the generic path compiles to LD.E / ST.E)
+__device__ __forceinline__ void sts64(uint32_t addr, float a, float b) {
+    asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(a), "f"(b) : "memory");
 }
 __device__ __forceinline__ float4 lds128(uint32_t addr) {
     float4 v;
     asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr) : "memory");
     return v;
 }
-__device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
-__device__ __forceinline__ void tmem_alloc(uint32_t dst_smem, uint32_t cols) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(cols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int PENDING>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(PENDING) : "memory"); }
+// keeps the compiler from touching accumulator registers across wgmma issue / wait points
+template <int R>
+__device__ __forceinline__ void fence_acc(float (&d)[R]) {
+#pragma unroll
+    for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t cols) {
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(cols) : "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem desc]      (TS mode, CTA pair: M = 256 over two SMs, each supplies half of B)
-__device__ __forceinline__ void umma_f16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], [%1], %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate) : "memory");
-}
-// same, kind::tf32: A (TMEM) and B (smem) hold fp32 bit patterns, the tensor core uses their top 19 bits (sign, 8-bit exponent,
-// 10-bit mantissa: the low 13 mantissa bits are ignored, i.e. operands are TRUNCATED to TF32), K = 8 per instruction
-__device__ __forceinline__ void umma_tf32_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::tf32 [%0], [%1], %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate) : "memory");
-}
-// smem (matrix descriptor: 128 rows x 32 B slice) -> TMEM (128 lanes x 8 columns)
-__device__ __forceinline__ void tmem_cp_128x256b(uint32_t taddr, uint64_t desc) {
-    asm volatile("tcgen05.cp.cta_group::2.128x256b [%0], %1;" ::"r"(taddr), "l"(desc) : "memory");
-}
-// arrive (once the issuing thread's prior MMAs retire) on the barrier at this offset in every CTA of `mask`
-__device__ __forceinline__ void umma_commit_mc(uint32_t bar, uint16_t mask) {
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-                 ::"r"(bar), "h"(mask) : "memory");
-}
-__device__ __forceinline__ void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t* r) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-          "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-          "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr) : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-// K-major SWIZZLE_128B shared-memory matrix descriptor (cute::UMMA::SmemDescriptor bit layout):
-//   [0,14) start address >> 4 | [16,30) LBO >> 4 | [32,46) SBO >> 4 | [46,48) version = 1 | [61,64) layout = 2
-// rows are 128 B (64 fp16) apart, 8-row groups (one swizzle atom) 1024 B apart.
+
+// K-major SWIZZLE_128B shared-memory matrix descriptor (wgmma):
+//   [0,14) start address >> 4 | [16,30) LBO >> 4 (unused for swizzled K-major) | [32,46) SBO >> 4 | [62,64) layout = 1 (128B)
+// rows are 128 B apart, 8-row groups (one swizzle atom) 1024 B apart; the tile base is 1024-byte aligned. The K slice of step
+// k inside the 128-byte row starts k x 32 B further (16 fp16 | 8 fp32), i.e. descriptor + 2 k.
 __device__ __forceinline__ uint64_t make_kmajor_sw128_desc(uint32_t smem_addr) {
     uint64_t d = 0;
     d |= (uint64_t)((smem_addr & 0x3FFFFu) >> 4);
-    d |= (uint64_t)1 << 16;                  // LBO (unused for swizzled K-major; canonical value)
-    d |= (uint64_t)(1024 >> 4) << 32;        // SBO
-    d |= (uint64_t)1 << 46;                  // descriptor version (Blackwell)
-    d |= (uint64_t)2 << 61;                  // SWIZZLE_128B
+    d |= (uint64_t)1 << 16;
+    d |= (uint64_t)(1024 >> 4) << 32;
+    d |= (uint64_t)1 << 62;
     return d;
 }
-// kind::f16 instruction descriptor (cute::UMMA::InstrDescriptor): D fp32, A/B fp16, both K-major, M x N
-__host__ __device__ constexpr uint32_t make_idesc_f16(int m, int n) {
-    return (1u << 4) | (0u << 7) | (0u << 10) | (0u << 15) | (0u << 16) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(m >> 4) << 24);
-}
 
-// kind::tf32 instruction descriptor: D fp32 (c_format 1), A / B TF32 (format 2), both K-major
-__host__ __device__ constexpr uint32_t make_idesc_tf32(int m, int n) {
-    return (1u << 4) | (2u << 7) | (2u << 10) | (0u << 15) | (0u << 16) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(m >> 4) << 24);
-}
-
-
-// ---- cta_group::1 variants (one CTA owns its tile) ---------------------------------------------------------------------
-__device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-        ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1) : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_1cta(uint32_t dst_smem, uint32_t cols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(cols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_1cta(uint32_t taddr, uint32_t cols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(cols) : "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc], kind::tf32 (operands truncated to TF32 by the tensor core), SS mode
-__device__ __forceinline__ void umma_tf32_ss(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate) : "memory");
-}
-// arrive on a CTA-local mbarrier once the issuing thread's prior MMAs retire
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void prefetch_tmap(const CUtensorMap* map) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
-}
-
-// ---- CTA-pair variants with both operands in shared memory (csrc/gru_conv_tc.cu, csrc/conv_tc.cu) ----------------------------
-__device__ __forceinline__ void tma_load_2d_2cta(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-        ::"r"(dst), "l"(map), "r"(bar & PEER_BIT_MASK), "r"(c0), "r"(c1) : "memory");
-}
-__device__ __forceinline__ void umma_f16_ss2(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(da), "l"(db), "r"(idesc), "r"(accumulate) : "memory");
+// Stage a warpgroup's m64nN accumulator fragment as fp32 rows of `pitch` bytes with the 16-byte chunk c of row r stored at
+// chunk c ^ (r & 7) (the layout the epilogues read back with lds128). `base` is the warpgroup's row 0.
+template <int N>
+__device__ __forceinline__ void stage_acc_rows(uint32_t base, int pitch, const float (&d)[N / 2], int col0) {
+    const int lane = threadIdx.x & 31, wr = ((threadIdx.x >> 5) & 3) * 16 + (lane >> 2);
+#pragma unroll
+    for (int i = 0; i < N / 2; i += 2) {
+        const int r = wr + 8 * ((i >> 1) & 1), c = col0 + 8 * (i >> 2) + 2 * (lane & 3);
+        sts64(base + r * pitch + (((c >> 2) ^ (r & 7)) << 4) + (c & 3) * 4, d[i], d[i + 1]);
+    }
 }
 
 // ---- profiling aid: in-stream timeline (globaltimer) of the tensor-core kernels --------------------------------------------

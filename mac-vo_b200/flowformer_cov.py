@@ -20,7 +20,7 @@ the class is checked against the reference network's golden outputs on the CPU. 
 * `corr_fn(f1, f2) -> (B, 1, H1, W1, H1, W1)`   all-pairs correlation volume (encoder.py:256-275)
 * `lookup_fn(cost_maps, coords) -> (B, 81, H1, W1)`  9x9 window lookup (decoder.py:141-153)
 
-By default both bind to the sm_100a CUDA kernels behind the C-ABI (`ops.corr_build`, `ops.corr_lookup`)
+By default both bind to the sm_90a CUDA kernels behind the C-ABI (`ops.corr_build`, `ops.corr_lookup`)
 and fail loudly when the library / a GPU is missing. Tests inject the CPU oracle instead.
 
 Restructuring relative to the reference (same arithmetic per output, fewer launches / bytes):
@@ -247,7 +247,7 @@ class FlowFormerCovNet:
                  lookup_fn: Callable[[Tensor, Tensor], Tensor] | None = None):
         self.device = torch.device(device)
         self.enc_dtype, self.dec_dtype, self.depth = enc_dtype, dec_dtype, decoder_depth
-        # TF32 mode only: SepConvGRU on the tcgen05 kernel (False / MACVO_B200_GRU_TC=0: cuDNN convolutions + glue kernels)
+        # TF32 mode only: SepConvGRU on the tensor-core kernel (False / MACVO_B200_GRU_TC=0: cuDNN convolutions + glue kernels)
         self.gru_tensor_cores = os.environ.get("MACVO_B200_GRU_TC", "1") != "0"
         self.conv_tensor_cores = os.environ.get("MACVO_B200_CONV_TC", "1") != "0"      # same, the decoder's 3x3 / 1x1 convolutions
         self.gru_split_units = os.environ.get("MACVO_B200_GRU_SPLIT", "1") != "0"      # one launch chain per GRU unit on two streams
@@ -725,7 +725,7 @@ class FlowFormerCovNet:
         gamma = self.W[ub + "aggregator.gamma"]
         P = B * N
         native = self._native(ctx) and dd == torch.float32
-        # TF32 mode: both SepConvGRU units run on the tcgen05 kernel (fp16 operands, fp32 state; csrc/gru_conv_tc.cu);
+        # TF32 mode: both SepConvGRU units run on the tensor-core kernel (fp16 operands, fp32 state; csrc/gru_conv_tc.cu);
         # strict mode keeps cuDNN's fp32 convolutions + the fused glue kernels
         gru_tc = dec_tc = None
         if native:
@@ -771,7 +771,7 @@ class FlowFormerCovNet:
         for _ in range(self.depth):
             if use_tc:
                 # TF32 mode: the whole iteration on our kernels — lookup, token kernel, motion encoder / value projection / heads
-                # on the tcgen05 convolution kernel (fp16 rows between the layers), SepConvGRU on its tcgen05 kernel; the one
+                # on the tensor-core convolution kernel (fp16 rows between the layers), SepConvGRU on its tensor-core kernel; the one
                 # library call left is the GMA aggregation GEMM
                 ops, t, shp = self._ops, dec_tc, (B, H1, W1)
                 main = torch.cuda.current_stream()
@@ -871,7 +871,7 @@ class FlowFormerCovNet:
                 agg = torch.matmul(attention, v)                                    # (B, N, 128) = pixels-major
             if native:
                 # the flow branch (GRU + flow head) and the covariance branch (GRU + cov head) only share their input:
-                # at 60x80 each conv fills about half of the 148 SMs, so the two run on forked streams (fork/join is
+                # at 60x80 each conv fills about two thirds of the 132 SMs, so the two run on forked streams (fork/join is
                 # captured into the CUDA graph as parallel branches)
                 if gru_tc is not None:
                     gru_tc.step(mf.permute(0, 2, 3, 1), agg, gamma)              # both units, 5 launches

@@ -5,7 +5,7 @@ Utility/Extensions/SubclassRegistry.py:25-48). When the MAC-VO tree is importabl
 the B200 plugins subclass MAC-VO's OWN interfaces, so importing `macvo_b200.plugins` registers them and a
 YAML `type: B200_...` selects them — `Odometry/MACVO.py` stays unchanged.
 
-When MAC-VO is not importable (the GPU box of this build has no reference tree) the minimal mirrors below
+When MAC-VO is not importable (no MAC-VO tree on the path) the minimal mirrors below
 provide the same names, signatures and error behaviour for the methods the hot path uses:
 
     IFrontend            Module/Frontend/Frontend.py:38-118

@@ -1,7 +1,7 @@
 """ctypes binding of libmacvo_b200.so (the C ABI in include/macvo_b200.h) for torch CUDA tensors.
 
 PyTorch only supplies device memory and the current stream here; every operator below is a
-hand-written sm_100a kernel. There is NO CPU / eager fallback: if the library is missing or the
+hand-written sm_90a kernel. There is NO CPU / eager fallback: if the library is missing or the
 tensors are not on a CUDA device the call raises.
 """
 from __future__ import annotations
@@ -174,7 +174,7 @@ def _workspace(key, nbytes: int, device) -> Tensor:
 def default_corr_mode(dim: int, n: int) -> int:
     """Strict fp32 (allow_tf32 off): the fp32-class 3 x fp16 split. With TF32 matmuls allowed — the reference frontend's
     own setting (Frontend.py:275-277), under which ITS `torch.matmul` for this product runs on TF32 tensor cores — one
-    kind::tf32 pass straight over the fp32 features (no operand pre-pass)."""
+    tf32 pass straight over the fp32 features (no operand pre-pass)."""
     env = os.environ.get("MACVO_B200_CORR_MODE")
     if env is not None:
         return {"simt": CORR_SIMT, "tc3": CORR_TC_3XF16, "tc1": CORR_TC_1XF16, "tf32": CORR_TC_TF32}[env]
@@ -913,7 +913,7 @@ def pack_conv_filter(weight: Tensor, bias: Tensor | None, in_channels: int | Non
 def conv_tc(in_rows: Tensor, weights: Tensor, bias: Tensor | None, n_valid: int, ksize: int, relu: bool, shape: tuple[int, int, int],
             in_dense: bool = False, out16: Tensor | None = None, out16_offset: int = 0, out16_dense: bool = False,
             out32: Tensor | None = None, out32_offset: int = 0, add_to_map: Tensor | None = None) -> None:
-    """3x3 / 1x1 convolution on the tcgen05 path (csrc/conv_tc.cu): fp16 pixel rows in, fp16 rows and / or fp32 dense rows out;
+    """3x3 / 1x1 convolution on the tensor-core path (csrc/conv_tc.cu): fp16 pixel rows in, fp16 rows and / or fp32 dense rows out;
     `add_to_map` (B, n_valid, H, W) fp32 instead of out32: the result is added to that map in place"""
     B, H, W = shape
     for t, dt, what in ((in_rows, torch.float16, "in_rows"), (weights, torch.float16, "weights"), (out16, torch.float16, "out16"),
@@ -965,7 +965,7 @@ def pack_rows(src: Tensor, dst: Tensor, offset: int, shape: tuple[int, int, int]
 
 
 class SepConvGruTC:
-    """The decoder's SepConvGRU units (gru.py:22-43; flow + covariance, covhead.py:95-131) on the tcgen05 path
+    """The decoder's SepConvGRU units (gru.py:22-43; flow + covariance, covhead.py:95-131) on the tensor-core path
     (csrc/gru_conv_tc.cu): fp32 recurrent state `h[u]` (pixels, 128) in dense pixel order, fp16 padded operand rows for the two
     passes, one `step` = pack the motion features + 4 kernel launches for all units.
 
@@ -1028,7 +1028,7 @@ class SepConvGruTC:
     def step(self, mf: Tensor, agg: Tensor, gamma: Tensor, split_units: bool = False, join: bool = True):
         """one SepConvGRU update of every unit with x = [inp | mf | mf + gamma * agg]; new state in `self.h[u]`.
         split_units: one 4-launch chain per unit on two streams instead of 4 launches covering both units — with 84 CTA tiles per
-        unit (640x480: two 60x80 maps) a joint launch is 168 CTAs = two waves on 148 SMs per stage, two independent chains of
+        unit (640x480: two 60x80 maps) a joint launch is 168 CTAs = two waves on 132 SMs per stage, two independent chains of
         84-CTA launches keep the SMs filled across the stage boundaries. With join=False the current stream only carries
         unit 0's chain and the returned event marks the end of unit 1's (the caller orders unit 1's consumers after it)."""
         B, H, W = self.shape

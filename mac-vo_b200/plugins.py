@@ -62,7 +62,7 @@ def _require_cuda(device: str, who: str) -> torch.device:
 # Frontend
 # ================================================================================================
 class B200_FlowFormerCovFrontend(IFrontend):
-    """FlowFormerCov stereo + flow frontend: correlation volume and window lookup on sm_100a kernels,
+    """FlowFormerCov stereo + flow frontend: correlation volume and window lookup on sm_90a kernels,
     dense post-processing + keypoint scoring fused into one pass, the whole `estimate_pair` replayed as a
     CUDA graph (like CUDAGraph_FlowFormerCovFrontend, Frontend.py:301-353).
 
@@ -81,8 +81,8 @@ class B200_FlowFormerCovFrontend(IFrontend):
             sd = torch.load(w, map_location="cpu", weights_only=True)
         enc, dec = _DTYPES[config.enc_dtype], _DTYPES[config.dec_dtype]
         # MACVO_Fast (enc fp16 / dec bf16, Config/Experiment/MACVO/MACVO_Fast.yaml:8-9) exists because half-precision tensor
-        # cores are the fast path on the GPUs MAC-VO targets. On B200 the TF32 pipeline of this class (own kernels + TF32
-        # cuDNN / cuBLAS) is both faster than a half-precision torch-op network and ~4x closer to exact arithmetic than the
+        # cores are the fast path on the GPUs MAC-VO targets. The TF32 pipeline of this class (own kernels + TF32
+        # cuDNN / cuBLAS) is ~4x closer to exact arithmetic than the
         # reference's own fp16 / bf16 run (flow 9e-4 vs 3.3e-3 of its scale, tests/test_gpu_pipeline.py::test_fast_config_*),
         # so half-precision configs are served by it unless `half_precision: native` asks for the literal dtypes.
         self.half_precision = getattr(config, "half_precision", "tf32")

@@ -1,5 +1,5 @@
 """TEST INFRASTRUCTURE — restatement of the parts of `pypose` (pinned by the reference at
-pypose==0.6.8, `static_analysis_requirements.txt:1`; source NOT under /root/reference, not
+pypose==0.6.8, `static_analysis_requirements.txt:1`; source NOT in the MAC-VO tree, not
 installed, no network) that MAC-VO's two-frame pose-graph path touches.
 
 Only `tests/`, `tests/golden/make_golden.py`, `__graft_entry__.smoke()` and `bench.py`'s CPU legs

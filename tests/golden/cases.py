@@ -1,5 +1,5 @@
-"""Seeded synthetic inputs shared by tests/golden/make_golden.py (reference side, build container)
-and the parity tests (oracle / CUDA side, also on the GPU box). SURVEY.md §8(d) shapes.
+"""Seeded synthetic inputs shared by tests/golden/make_golden.py (reference side)
+and the parity tests (oracle / CUDA side). SURVEY.md §8(d) shapes.
 
 Only CPU torch generators and EXACTLY ROUNDED operations (+, -, *, round, table look-ups) are used -> identical bits
 wherever the same torch build runs. No transcendental functions: round 1's generators used `torch.exp(torch.randn(..))`

@@ -1,8 +1,8 @@
 """Generate the golden fixtures under tests/golden/ by running the REFERENCE ITSELF on CPU.
 
-Run in the build container only (needs /root/reference):  python tests/golden/make_golden.py
-The fixtures are small `.pt` files holding seeded inputs + the reference's outputs; the GPU box
-(which has no /root/reference) only reads them. Everything is seeded -> re-running reproduces
+Needs a MAC-VO checkout:  MACVO_REFERENCE_ROOT=<MAC-VO checkout> python tests/golden/make_golden.py
+The fixtures are small `.pt` files holding seeded inputs + the reference's outputs; the tests
+(which never need the MAC-VO tree) only read them. Everything is seeded -> re-running reproduces
 the files bit-for-bit on the same torch build.
 
 What executes here is the unmodified reference code:

@@ -1,6 +1,6 @@
 """Generate tests/golden/net_cfgA.pt: the 640x480, decoder_depth 12 parity fixture (BASELINE configs[1] shape).
 
-Run in the build container only (needs /root/reference, ~2.5 min):  python tests/golden/make_golden_cfgA.py
+Needs a MAC-VO checkout (~2.5 min):  MACVO_REFERENCE_ROOT=<MAC-VO checkout> python tests/golden/make_golden_cfgA.py
 
 Contents (strided samples, tests/golden/cases.py::cfgA_sample):
   ref32   flow / cov of the UNMODIFIED reference network (`FlowFormerCov.inference`, flownet.py:37-44) in fp32 on the CPU;

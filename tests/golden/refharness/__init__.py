@@ -1,7 +1,7 @@
-"""TEST INFRASTRUCTURE: import the read-only MAC-VO reference (`/root/reference`) in this container.
+"""TEST INFRASTRUCTURE: import a read-only MAC-VO source tree (MACVO_REFERENCE_ROOT, default `/root/reference`).
 
 Used only by `tests/golden/make_golden.py` (fixture generation) and by tests that are skipped when
-`/root/reference` is absent (it never exists on the GPU box). Nothing in the product imports this.
+no MAC-VO tree is found there. Nothing in the product imports this.
 
 * `yacs` is absent -> tiny `CfgNode` stand-in (`refharness/yacs`).
 * `pypose` is absent -> functional restatement (`oracle/pypose_shim`).

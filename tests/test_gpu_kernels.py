@@ -1,4 +1,4 @@
-"""GPU parity tests (B200): every CUDA kernel, called through the C ABI (macvo_b200.ops -> ctypes),
+"""GPU parity tests (H100): every CUDA kernel, called through the C ABI (macvo_b200.ops -> ctypes),
 against the CPU oracle on the same seeded inputs and against the committed golden fixtures.
 
 Tolerances (written next to each assert):
@@ -66,7 +66,7 @@ def test_corr_simt_matches_oracle_and_golden(ops, golden, name):
 
 @pytest.mark.parametrize("shape", [(2, 12, 16), (1, 30, 40), (2, 60, 80), (1, 80, 80), (1, 9, 13)])
 def test_corr_tensor_core_3xf16(ops, shape):
-    """tcgen05 kernel, fp32-class accuracy via the fp16 hi/lo split; incl. ragged M/N tile edges."""
+    """wgmma kernel, fp32-class accuracy via the fp16 hi/lo split; incl. ragged M/N tile edges."""
     B, H1, W1 = shape
     f1, f2 = cases.corr_inputs(B, H1, W1)
     if (H1 * W1) % 8:
@@ -83,7 +83,7 @@ def test_corr_tensor_core_3xf16(ops, shape):
 @pytest.mark.parametrize("shape", [(2, 12, 16), (1, 30, 40), (2, 60, 80), (1, 80, 80), (1, 9, 13), (1, 90, 160)])
 @pytest.mark.parametrize("layout", ["channels_last", "nchw"])
 def test_corr_tensor_core_tf32(ops, shape, layout):
-    """tcgen05 kind::tf32, one pass straight over the fp32 K-major features (the mode used when TF32 matmuls are allowed,
+    """wgmma tf32, one pass straight over the fp32 K-major features (the mode used when TF32 matmuls are allowed,
     like the reference's own torch.matmul under Frontend.py:275-277). Operands are truncated to 10 mantissa bits by the
     tensor core: |err| <= 2^-9 |f1_i| |f2_j| worst case; asserted at 6e-4 (measured ~2e-4 over 23 M entries), and the
     result must equal an fp64 product of the TRUNCATED operands to fp32 accumulation accuracy (2e-6): that pins the

@@ -131,7 +131,7 @@ def test_gru_fused_kernels(ops):
 
 @pytest.mark.parametrize("shape", [(1, 60, 80), (1, 12, 16), (2, 13, 17), (1, 90, 160)])
 def test_sepconv_gru_tensor_cores(ops, shape):
-    """csrc/gru_conv_tc.cu (tcgen05 implicit GEMM, fp16 operands, fp32 state) vs SepConvGRU (core/gru.py:22-43) in float64:
+    """csrc/gru_conv_tc.cu (wgmma implicit GEMM, fp16 operands, fp32 state) vs SepConvGRU (core/gru.py:22-43) in float64:
     (a) against the same arithmetic with the convolution inputs / filters rounded to fp16 (what the kernel computes): 1e-3,
     (b) against the unrounded float64 GRU: 4e-3 (fp16 operand rounding, the TF32-class bound of this mode). Two steps, two units,
     so the layout ping-pong between the 1x5 and the 5x1 pass and the state hand-over to the next iteration are covered."""

@@ -32,7 +32,7 @@ def _strict_fp32():
 
 @pytest.mark.parametrize("name", list(cases.NET_CASES))
 def test_network_with_cuda_kernels_matches_reference_golden(plugins, golden, name):
-    """FlowFormerCov with the sm_100a corr + lookup kernels vs the REFERENCE network's CPU output (golden).
+    """FlowFormerCov with the sm_90a corr + lookup kernels vs the REFERENCE network's CPU output (golden).
     fp32, TF32 off. The reference's own fp32 result sits ~1e-6 (flow) / ~2e-5 (covariance) from exact arithmetic at these
     sizes (tests/golden/make_golden_cfgA.py measures the same floor at 640x480); asserted: 2e-5 of the flow scale and 3e-4
     relative on the covariance. The 640x480 / depth-12 ladder in both precision modes is tests/test_gpu_parity_ladder.py."""

@@ -1,5 +1,5 @@
-"""The five B200 plugin classes driven by the REAL, unmodified `Odometry/MACVO.py` (build container only: needs
-/root/reference; skipped elsewhere). YAML-shaped config -> `MACVO.from_config` -> registry -> 4 frames of `MACVO.run`
+"""The five B200 plugin classes driven by the REAL, unmodified `Odometry/MACVO.py` (needs a MAC-VO
+tree, see tests/golden/refharness; skipped elsewhere). YAML-shaped config -> `MACVO.from_config` -> registry -> 4 frames of `MACVO.run`
 (`initialize`, `run_pair`, `get_graph_data` -> `B200_TwoFrame_PGO._optimize(GraphInput)` -> `write_graph_data`,
 mapping branch) -> `terminate` (MotionInterpolate). No GPU here: every C-ABI call is answered by the CPU oracle
 (tests/mock_ops.py), so what this pins is the plugin HOST logic under MAC-VO's exact call pattern — the transposed

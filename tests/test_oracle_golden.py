@@ -1,5 +1,5 @@
 """The CPU oracle (oracle/) pinned against fixtures produced by the reference itself
-(tests/golden/make_golden.py). No GPU, no /root/reference needed."""
+(tests/golden/make_golden.py). No GPU, no MAC-VO tree needed."""
 import numpy as np
 import pytest
 import torch

@@ -1,4 +1,4 @@
-"""Drop-in check against the REAL MAC-VO tree (build container only; skipped where /root/reference is absent):
+"""Drop-in check against the REAL MAC-VO tree (skipped where no MAC-VO tree is found, see tests/golden/refharness):
 importing `macvo_b200.plugins` with MAC-VO importable registers the B200 classes in MAC-VO's own registries,
 `Module.I<X>.instantiate` finds them by name and `is_valid_config` accepts the INTEGRATION.md YAML args.
 Runs in a subprocess so that the reference import does not leak into the other tests."""

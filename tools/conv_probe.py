@@ -1,4 +1,4 @@
-"""Event trace + graph timing of one tcgen05 convolution (csrc/conv_tc.cu) at the decoder's shapes (B = 2, 60 x 80)."""
+"""Event trace + graph timing of one tensor-core (wgmma) convolution (csrc/conv_tc.cu) at the decoder's shapes (B = 2, 60 x 80)."""
 import json
 import os
 import sys

@@ -1,4 +1,4 @@
-"""Device time of the 12-iteration decoder alone (captured into a CUDA graph): tcgen05 convolutions + GRU vs GRU only vs cuDNN."""
+"""Device time of the 12-iteration decoder alone (captured into a CUDA graph): tensor-core convolutions + GRU vs GRU only vs cuDNN."""
 import json
 import os
 import sys

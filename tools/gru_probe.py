@@ -1,4 +1,4 @@
-"""Timing of one SepConvGRU update of both decoder units at 60x80: tcgen05 kernel path vs cuDNN + glue kernels."""
+"""Timing of one SepConvGRU update of both decoder units at 60x80: tensor-core (wgmma) kernel path vs cuDNN + glue kernels."""
 import json
 import sys
 import os
