@@ -440,6 +440,27 @@ size_t macvo_motion_interpolate_workspace_bytes(int num_frames);
 int macvo_motion_interpolate(float* poses, const uint8_t* need_interp, int num_frames, int* n_interp, void* workspace,
                              size_t workspace_bytes, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * (f5) TartanMotionNet pose network (VOFlowRes config 1, Module/Network/TartanVOStereo/FlowPoseNet.py:45-165).
+ *
+ * macvo_posenet_input: flow (2,H,W) + depth (1,H,W) fp32 (H >= 112, W >= 160) -> channels 0..2 of the (5,112,160) network
+ *      input `out` (channels 3..4, the intrinsics layer, are left untouched): TartanStereoVOMotion.inference
+ *      (StereoVO_Interface.py:158-194) — centre crop, bilinear align_corners resize, flow x 0.05, normalised disparity.
+ * macvo_posenet_conv: y = epilogue(conv(x, W) + bias [+ resid]) for x (cin,hi,wi), y (cout,ho,wo); epilogue = ReLU when
+ *      `relu`. w_packed (16-byte aligned) holds W (cout,cin,k,k) as per-CTA slabs [cout/co_tile][8][co_tile][cin/8*k*k];
+ *      cin % 8 == 0, cout % co_tile == 0, co_tile * cin/8 * k*k % 4 == 0. Deterministic (no atomics).
+ * macvo_posenet_head: fc1_out (256) = [trans 128 | rot 128] after ReLU; head_blob (macvo_posenet_head_floats()) =
+ *      [fc2 trans W (32x128) | b | fc2 rot W | b | fc3 trans W (3x32) | b | fc3 rot W | b | pose_norm (6)];
+ *      motion (6) fp32 = cat(trans, rot) * pose_norm; next_pose (7) float64 = prev_pose (rounded to fp32) @ se3(motion).Exp()
+ *      in fp32 ([t, q_xyzw]).
+ */
+int macvo_posenet_input(const float* flow, const float* depth, int height, int width, double bl_fx, float* out, void* stream);
+int macvo_posenet_conv(const float* x, int cin, int hi, int wi, const float* w_packed, const float* bias, int cout, int ksize,
+                       int stride, int pad, int co_tile, const float* resid, int relu, float* y, void* stream);
+size_t macvo_posenet_head_floats(void);
+int macvo_posenet_head(const float* fc1_out, const float* head_blob, const double* prev_pose, float* motion,
+                       double* next_pose, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

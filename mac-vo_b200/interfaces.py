@@ -13,6 +13,7 @@ provide the same names, signatures and error behaviour for the methods the hot p
     IMatcher.Output      Module/Frontend/Matching.py:23-40
     IKeypointSelector    Module/KeypointSelector.py:17-48
     ICovariance2to3      Module/Covariance/Project2to3.py:16-44
+    IMotionModel         Module/MotionModel.py:15-41
     IOptimizer           Module/Optimization/Interface.py:40-242 (sequential mode only)
     StereoData           DataLoader/Interface.py:57-113
     ConfigTestable._enforce_config_spec  Utility/Extensions/Testable.py:23-42
@@ -211,6 +212,21 @@ class IMapProcessor(ABC, _Registry):
 
     @abstractmethod
     def elaborate_map(self, frames): ...
+
+
+class IMotionModel(ABC, _Registry):
+    """Module/MotionModel.py:15-41: `predict` returns the pose of the incoming frame in world coordinates, `update`
+    receives the optimised pose of the previous frame."""
+    _IS_INTERFACE = True
+
+    def __init__(self, config: SimpleNamespace) -> None:
+        self.config = config
+
+    @abstractmethod
+    def predict(self, frame, flow: torch.Tensor | None, depth: torch.Tensor | None) -> torch.Tensor: ...
+
+    @abstractmethod
+    def update(self, pose: torch.Tensor) -> None: ...
 
 
 class IOptimizer(ABC, _Registry):

@@ -112,6 +112,11 @@ EXPORTS = {
     "macvo_gru_tc_stage": (C.c_int, [C.c_int] * 6 + [C.c_void_p] * 8),
     "macvo_gru_tc_pack": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p] + [C.c_int] * 6 + [C.c_void_p]),
     "macvo_gru_tc_pack_motion": (C.c_int, [C.c_void_p] * 5 + [C.c_int] * 3 + [C.c_void_p]),
+    "macvo_posenet_input": (C.c_int, [C.c_void_p] * 2 + [C.c_int] * 2 + [C.c_double, C.c_void_p, C.c_void_p]),
+    "macvo_posenet_conv": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int] + [C.c_void_p] * 2 + [C.c_int] * 5
+                           + [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
+    "macvo_posenet_head_floats": (C.c_size_t, []),
+    "macvo_posenet_head": (C.c_int, [C.c_void_p] * 6),
 }
 
 
@@ -1234,3 +1239,94 @@ def latent_pool(tokens: Tensor, q: Tensor, wk: Tensor, wv: Tensor, bv: Tensor) -
     _check(rc, "macvo_latent_pool")
     LAUNCHES[0] += 1
     return out
+
+
+# ------------------------------------------------------------------------------------------------
+# (f5) TartanMotionNet pose network (csrc/posenet.cu)
+# ------------------------------------------------------------------------------------------------
+POSENET_H, POSENET_W = 112, 160
+POSENET_SPLIT = 8           # K split of macvo_posenet_conv = its thread-block cluster size
+
+
+def posenet_co_tile(cout: int) -> int:
+    """output channels per CTA: cout / 32 tiles x 8 K-splits = 256 CTAs for every layer (two per SM on an H100)"""
+    return max(1, cout // 32)
+
+
+def pack_posenet_conv(weight: Tensor) -> tuple[Tensor, int]:
+    """(cout, cin, k, k) (or (cout, cin) for a linear layer) -> the per-CTA weight slabs macvo_posenet_conv streams:
+    [cout/co_tile][8][co_tile][cin/8 * k * k], each slab contiguous. Done once, at construction."""
+    w = weight.detach().float()
+    cout, cin = w.shape[:2]
+    if cin % POSENET_SPLIT:
+        raise MacvoB200Error(f"pack_posenet_conv: cin {cin} is not a multiple of {POSENET_SPLIT}")
+    ct = posenet_co_tile(cout)
+    kc = w[0].numel() // POSENET_SPLIT
+    packed = (w.reshape(cout // ct, ct, POSENET_SPLIT, kc).permute(0, 2, 1, 3).contiguous().reshape(-1))
+    return packed, ct
+
+
+def posenet_input(flow: Tensor, depth: Tensor, bl_fx: float, out: Tensor) -> None:
+    """channels 0..2 of the (1,5,112,160) pose-network input from flow (1,2,H,W) and depth (1,1,H,W)"""
+    fl = _dev(flow, torch.float32, "posenet_input flow")
+    dp = _dev(depth, torch.float32, "posenet_input depth")
+    H, W = fl.shape[-2:]
+    if fl.numel() != 2 * H * W or dp.numel() != H * W:
+        raise MacvoB200Error("posenet_input: expects flow (1,2,H,W) and depth (1,1,H,W)")
+    if H < POSENET_H or W < POSENET_W:
+        raise MacvoB200Error(f"posenet_input: maps of {H}x{W} are smaller than the network input {POSENET_H}x{POSENET_W}")
+    if not (out.is_cuda and out.dtype == torch.float32 and out.is_contiguous() and out.numel() == 5 * POSENET_H * POSENET_W):
+        raise MacvoB200Error("posenet_input: out must be a contiguous (1,5,112,160) fp32 CUDA tensor")
+    _check(load_library().macvo_posenet_input(fl.data_ptr(), dp.data_ptr(), H, W, float(bl_fx), out.data_ptr(), _stream()),
+           "macvo_posenet_input")
+    LAUNCHES[0] += 1
+
+
+def posenet_conv(x: Tensor, packed: Tensor, co_tile: int, bias: Tensor, ksize: int, stride: int, pad: int,
+                 resid: Tensor | None = None, relu: bool = False, out: Tensor | None = None) -> Tensor:
+    """epilogue(conv2d(x, W, bias, stride, pad) [+ resid]) for one image x (cin,hi,wi) (a leading batch of 1 is accepted);
+    W given as pack_posenet_conv's slabs. Returns (1, cout, ho, wo)."""
+    x = _dev(x, torch.float32, "posenet_conv x")
+    cin, hi, wi = x.shape[-3:]
+    if x.numel() != cin * hi * wi:
+        raise MacvoB200Error("posenet_conv: x must hold one image")
+    b = _dev(bias, torch.float32, "posenet_conv bias")
+    cout = b.numel()
+    pk = _dev(packed, torch.float32, "posenet_conv weights")
+    if pk.numel() != cout * cin * ksize * ksize:
+        raise MacvoB200Error(f"posenet_conv: {pk.numel()} packed weights for cout {cout}, cin {cin}, k {ksize}")
+    ho, wo = (hi + 2 * pad - ksize) // stride + 1, (wi + 2 * pad - ksize) // stride + 1
+    if out is None:
+        out = torch.empty((1, cout, ho, wo), dtype=torch.float32, device=x.device)
+    elif not (out.is_cuda and out.dtype == torch.float32 and out.is_contiguous() and out.numel() == cout * ho * wo):
+        raise MacvoB200Error("posenet_conv: out has the wrong shape")
+    r = None
+    if resid is not None:
+        r = _dev(resid, torch.float32, "posenet_conv resid")
+        if r.numel() != cout * ho * wo:
+            raise MacvoB200Error("posenet_conv: resid must have the output's shape")
+    rc = load_library().macvo_posenet_conv(x.data_ptr(), cin, hi, wi, pk.data_ptr(), b.data_ptr(), cout, ksize, stride, pad,
+                                           int(co_tile), r.data_ptr() if r is not None else None, int(bool(relu)),
+                                           out.data_ptr(), _stream())
+    _check(rc, "macvo_posenet_conv")
+    LAUNCHES[0] += 1
+    return out
+
+
+def posenet_head_floats() -> int:
+    return int(load_library().macvo_posenet_head_floats())
+
+
+def posenet_head(fc1_out: Tensor, head_blob: Tensor, prev_pose: Tensor, motion: Tensor, next_pose: Tensor) -> None:
+    """fc2 / fc3 of both heads x pose_norm -> motion (6,) fp32, and next_pose (7,) float64 = prev_pose @ se3(motion).Exp()"""
+    h = _dev(fc1_out, torch.float32, "posenet_head fc1_out")
+    blob = _dev(head_blob, torch.float32, "posenet_head blob")
+    pp = _dev(prev_pose, torch.float64, "posenet_head prev_pose")
+    if h.numel() != 256 or blob.numel() != posenet_head_floats() or pp.numel() != 7:
+        raise MacvoB200Error("posenet_head: expects fc1_out (256,), the head blob and prev_pose (7,)")
+    for t, dt, n, what in ((motion, torch.float32, 6, "motion"), (next_pose, torch.float64, 7, "next_pose")):
+        if not (t.is_cuda and t.dtype == dt and t.is_contiguous() and t.numel() == n):
+            raise MacvoB200Error(f"posenet_head: {what} must be a contiguous ({n},) {dt} CUDA tensor")
+    _check(load_library().macvo_posenet_head(h.data_ptr(), blob.data_ptr(), pp.data_ptr(), motion.data_ptr(),
+                                             next_pose.data_ptr(), _stream()), "macvo_posenet_head")
+    LAUNCHES[0] += 1

@@ -47,8 +47,9 @@ class TwoFrameOdometry:
 
     def __init__(self, frontend, kp_selector, cov_model, optimizer, num_point: int = 200, edgewidth: int = 32,
                  match_cov_default: float = 0.25, mapping: bool = True, map_selector=None, min_num_point: int = 10,
-                 keep_debug: bool = False):
+                 keep_debug: bool = False, motion_model=None):
         self.frontend, self.kp_selector, self.cov_model, self.optimizer = frontend, kp_selector, cov_model, optimizer
+        self.motion_model = motion_model            # None: StaticMotionModel (the prediction is the previous pose)
         self.map_selector = map_selector
         self.num_point, self.edgewidth, self.match_cov_default = num_point, edgewidth, match_cov_default
         self.mapping, self.min_num_point, self.keep_debug = mapping, min_num_point, keep_debug
@@ -61,6 +62,8 @@ class TwoFrameOdometry:
         depth0 = self.frontend.estimate_depth(frame0)
         self.prev = (frame0, depth0)
         self.poses = [torch.tensor([0., 0., 0., 0., 0., 0., 1.])]
+        if self.motion_model is not None:         # the first prediction is the identity (MACVO.initialize)
+            self.motion_model.predict(frame0, None, depth0.depth)
 
     def _write_back(self) -> None:
         """Optimizer.write_map (Odometry/MACVO.py:187): blocks on the previous frame's result."""
@@ -76,7 +79,12 @@ class TwoFrameOdometry:
         depth1, match01 = fe.estimate_pair(frame0, frame1)
         self._write_back()
         prev_pose = self.poses[-1]
-        est_pose = prev_pose.clone()                                   # StaticMotionModel.predict (MotionModel.py:133-137)
+        if self.motion_model is None:
+            est_pose = prev_pose.clone()                               # StaticMotionModel.predict (MotionModel.py:133-137)
+        else:                                                          # Odometry/MACVO.py:193-194
+            self.motion_model.update(prev_pose)
+            pred = self.motion_model.predict(frame1, match01.flow, depth1.depth)
+            est_pose = (pred.tensor() if hasattr(pred, "ltype") else pred).reshape(7).detach().cpu().float()
 
         kp0_uv = self.kp_selector.select_point(frame0, self.num_point, depth0, depth1, match01)
         kp1_uv = kp0_uv + fe.retrieve_pixels(kp0_uv, match01.flow).T
@@ -156,13 +164,19 @@ class FusedTwoFrameOdometry:
     with the plugin-API calls has >= 7 (candidate counts x2, boolean indexing x2, covariance `.cpu()` x3).
 
     Requires the B200 plugins (uses their device buffers); keypoints and poses equal `TwoFrameOdometry`'s
-    (tests/test_gpu_pipeline.py::test_fused_tail_matches_plugin_path)."""
+    (tests/test_gpu_pipeline.py::test_fused_tail_matches_plugin_path).
+
+    `motion_model` (a `plugins.B200_TartanMotionNet`, or None for the previous pose): its graph up to fc1 is enqueued right
+    after each frame's frontend, the prefetched next frame's included — it reads only that frame's flow and depth — and
+    its head kernel runs in the tail after observe_pack, overwriting the LM's initial pose with the prediction. No extra
+    host synchronisation."""
 
     def __init__(self, frontend, kp_selector, cov_model, optimizer, num_point: int = 200, edgewidth: int = 32,
                  match_cov_default: float = 0.25, mapping: bool = True, map_selector=None, min_num_point: int = 10,
-                 num_map_point: int = 2000, keep_debug: bool = False, solver=None):
+                 num_map_point: int = 2000, keep_debug: bool = False, solver=None, motion_model=None):
         from . import ops
         self.ops = ops
+        self.motion_model = motion_model
         # solver(obs, intr5, pose_io, stats, min_k): the LM solve on the packed observation buffer; default = one persistent
         # launch on this GPU. bench.py --config sharded plugs in the multi-GPU solve (broadcast + sharded_pgo.FusedShardedPGO)
         self.solver = solver
@@ -213,9 +227,10 @@ class FusedTwoFrameOdometry:
         frame0, depth0 = self.prev
         slot = self.frame_no & 1
         if self._prefetched is not None and self._prefetched[0] is frame1:
-            depth1, match01 = self._prefetched[1:]
+            depth1, match01, fc1 = self._prefetched[1:]
         else:
             depth1, match01 = self.frontend.estimate_pair(frame0, frame1)
+            fc1 = self._enqueue_motion(frame1, depth1, match01)
         self._prefetched = None
         main = torch.cuda.current_stream()
         if self._tail_done is not None:            # the previous frame's tail read the candidate lists the selectors now overwrite
@@ -227,22 +242,31 @@ class FusedTwoFrameOdometry:
         counts = ops.request_candidate_counts(reqs)
         if next_frame is None:
             counts.synchronize()
-            return self._tail(frame0, frame1, depth0, depth1, match01, reqs, slot)
-        self._prefetched = (next_frame, *self.frontend.estimate_pair(frame1, next_frame))
+            return self._tail(frame0, frame1, depth0, depth1, match01, reqs, slot, fc1)
+        d_next, m_next = self.frontend.estimate_pair(frame1, next_frame)
+        self._prefetched = (next_frame, d_next, m_next, self._enqueue_motion(next_frame, d_next, m_next))
         counts.synchronize()
         if self._tail_stream is None:
             self._tail_stream = torch.cuda.Stream(self.device)
         tail = self._tail_stream
         tail.wait_event(counts)
-        for t in (match01.flow, match01.cov, depth0.depth, depth1.depth, depth1.disparity, depth1.disparity_uncertainty):
-            t.record_stream(tail)              # allocated on the main stream, consumed on the tail stream
+        for t in (match01.flow, match01.cov, depth0.depth, depth1.depth, depth1.disparity, depth1.disparity_uncertainty, fc1):
+            if t is not None:
+                t.record_stream(tail)          # allocated on the main stream, consumed on the tail stream
         with torch.cuda.stream(tail):
-            res = self._tail(frame0, frame1, depth0, depth1, match01, reqs, slot)
+            res = self._tail(frame0, frame1, depth0, depth1, match01, reqs, slot, fc1)
             self._tail_done = torch.cuda.Event()
             self._tail_done.record(tail)
         return res
 
-    def _tail(self, frame0, frame1, depth0, depth1, match01, reqs, slot) -> FrameResult:
+    def _enqueue_motion(self, frame1, depth1, match01):
+        """the motion model's graph (input builder .. fc1) for this frame; its fc1 output copied out of the graph's static
+        buffer, which the prefetched next frame's replay overwrites before this frame's tail reads it"""
+        if self.motion_model is None:
+            return None
+        return self.motion_model.enqueue(frame1, match01.flow, depth1.depth).clone()
+
+    def _tail(self, frame0, frame1, depth0, depth1, match01, reqs, slot, fc1=None) -> FrameResult:
         """everything after the candidate counts reached the host, on the current stream"""
         ops = self.ops
         picks = ops.sample_from_counts(reqs)
@@ -253,6 +277,9 @@ class FusedTwoFrameOdometry:
         ops.observe_pack(obs, kp0_uv, match01.flow, match01.cov, depth0.depth, depth1.depth, depth1.disparity,
                          depth1.disparity_uncertainty, self.edgewidth, i0, i1, self.pose_dev[-1], next_pose,
                          match_cov_default=self.match_cov_default, **self.cov_args)
+        if fc1 is not None:     # the motion model's prediction replaces observe_pack's previous-pose prior
+            self.motion_model.head(fc1, self.pose_dev[-1], next_pose)
+        pose_init = next_pose.clone() if self.keep_debug else None      # the LM's initial pose, before the solve
         bl = float(torch.as_tensor(frame1.frame_baseline, dtype=torch.float32).double().reshape(-1)[0])
         stats.zero_()
         if self.solver is not None:
@@ -283,7 +310,7 @@ class FusedTwoFrameOdometry:
         res = FrameResult(num_kp=-1, num_obs=-1, pose_init=None, optimizer_output=None, map_points=n_map)
         if self.keep_debug:
             res.kp0_uv = kp0_uv
-            res.extras = {"depth1": depth1, "match01": match01, "slot": slot}
+            res.extras = {"depth1": depth1, "match01": match01, "slot": slot, "pose_init": pose_init}
         self.last = res
         return res
 

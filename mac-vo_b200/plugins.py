@@ -8,6 +8,7 @@
     B200_CovarianceSanityFilter      IObservationFilter replaces CovarianceSanityFilter (OutlierFilter.py:91-100)
     B200_MotionInterpolate           IMapProcessor      replaces MotionInterpolate (MapProcessor.py:52-79)
     B200_TwoFrame_PGO                IOptimizer         replaces TwoFrame_PGO (Optimization/TwoFramePGO/Optimizer.py:23-108)
+    B200_TartanMotionNet             IMotionModel       replaces TartanMotionNet (MotionModel.py:89-116)
 
 Same constructor signature (`__init__(config: SimpleNamespace)`), same `is_valid_config` contract
 (unknown keys are an error), same argument meaning and return types as the classes they replace; class
@@ -27,6 +28,7 @@ import torch
 
 from . import interfaces as _local
 from . import ops
+from . import posenet
 from .flowformer_cov import FlowFormerCovNet, synthetic_state_dict
 
 _REF = _local.reference_available()
@@ -41,12 +43,16 @@ if _REF:   # subclass MAC-VO's own interfaces so that importing this module regi
     from Module.MapProcessor import IMapProcessor  # type: ignore
     from Module.Optimization.TwoFramePGO.Optimizer import TwoFrame_PGO as _PGOBase  # type: ignore
     from Module.Optimization.TwoFramePGO.Graphs import GraphOutput as _RefGraphOutput  # type: ignore
+    from Module.MotionModel import IMotionModel  # type: ignore
+    import pypose as _pp  # type: ignore
 else:
     StereoData = _local.StereoData
     IFrontend, IStereoDepth, IMatcher = _local.IFrontend, _local.IStereoDepth, _local.IMatcher
     IKeypointSelector, ICovariance2to3 = _local.IKeypointSelector, _local.ICovariance2to3
     IObservationFilter, IMapProcessor = _local.IObservationFilter, _local.IMapProcessor
     _PGOBase = _local.IOptimizer
+    IMotionModel = _local.IMotionModel
+    _pp = None
 
 _DTYPES = {"fp32": torch.float32, "fp16": torch.float16, "bf16": torch.bfloat16}
 
@@ -560,6 +566,117 @@ class B200_TwoFrame_PGO(_PGOBase):
             })
 
 
+# ================================================================================================
+# Motion model
+# ================================================================================================
+class B200_TartanMotionNet(IMotionModel):
+    """Replacement of TartanMotionNet (Module/MotionModel.py:89-116) that builds only the pose network `predict` runs
+    (no PWC-Net, no stereo net, no cupy / cv2). Everything from the flow and depth maps up to fc1 is one CUDA graph,
+    captured on the first prediction and replayed after; the head kernel (fc2 / fc3, pose composition) runs after the
+    replay because it reads the previous pose.
+
+    config: weight (checkpoint path — only its `module.flowPoseNet.*` tensors are used — or "synthetic[:seed]"), device.
+    `predict` returns identity on its first call, then prev_pose @ se3(motion).Exp() on the device: a pp.SE3 when MAC-VO
+    (and pypose) is importable, else a (7,) tensor [t, q_xyzw]."""
+
+    def __init__(self, config: SimpleNamespace):
+        super().__init__(config)
+        self.device = _require_cuda(config.device, "B200_TartanMotionNet")
+        w = config.weight
+        if isinstance(w, str) and w.startswith("synthetic"):
+            sd = posenet.synthetic_posenet_state_dict(int(w.split(":")[1]) if ":" in w else 0)
+        else:
+            sd = posenet.load_checkpoint(w)
+        self.net = posenet.PoseNet(sd, self.device)
+        self.prev_pose: torch.Tensor | None = None       # (7,) fp32 on the device
+        self.motion = torch.zeros((6,), dtype=torch.float32, device=self.device)   # last predicted se3 motion
+        self._replay = None
+        self._static: dict = {}
+
+    @staticmethod
+    def _camera(frame):
+        meta = getattr(frame, "stereo", frame)
+        return meta, (float(meta.fx), float(meta.fy), float(meta.cx), float(meta.cy)), meta.frame_baseline * meta.fx
+
+    @torch.inference_mode()
+    def enqueue(self, frame, flow: torch.Tensor, depth: torch.Tensor) -> torch.Tensor:
+        """Replay the graph (input builder .. fc1) for this frame's flow (1,2,H,W) and depth (1,1,H,W); returns the graph's
+        static fc1 output (256,), valid until the next call. Kernels only, no host synchronisation."""
+        meta, K, bl_fx = self._camera(frame)
+        st = self._static
+        if self._replay is not None:
+            assert tuple(flow.shape) == st["flow"].shape and tuple(depth.shape) == st["depth"].shape, \
+                f"map shape changed since the CUDA graph was captured: {tuple(flow.shape)} != {tuple(st['flow'].shape)}"
+            assert K == st["K"], "camera intrinsics changed since the CUDA graph was captured"
+            assert bl_fx == st["bl_fx"], "camera baseline * fx changed since the CUDA graph was captured"
+            st["flow"].copy_(flow, non_blocking=True)
+            st["depth"].copy_(depth, non_blocking=True)
+            return self._replay()
+        sflow = flow.to(device=self.device, dtype=torch.float32).contiguous().clone()
+        sdepth = depth.to(device=self.device, dtype=torch.float32).contiguous().clone()
+        inp = torch.empty((1, 5, ops.POSENET_H, ops.POSENET_W), dtype=torch.float32, device=self.device)
+        inp[:, 3:5] = posenet.intrinsic_layer(meta.height, meta.width, *K[:2], *K[2:], self.device)
+
+        def run():
+            ops.posenet_input(sflow, sdepth, bl_fx, inp)
+            return self.net.body(inp)
+        self._static = {"flow": sflow, "depth": sdepth, "inp": inp, "K": K, "bl_fx": bl_fx}
+        self._replay = self._capture(run)
+        return self._replay()
+
+    def _capture(self, run):
+        """capture `run` (input builder .. fc1) as a CUDA graph; returns a callable that replays it and returns fc1"""
+        side = torch.cuda.Stream(self.device)      # warm-up (cuDNN algorithm choice) outside the capture
+        side.wait_stream(torch.cuda.current_stream())
+        with torch.cuda.stream(side):
+            run()
+        torch.cuda.current_stream().wait_stream(side)
+        graph = torch.cuda.CUDAGraph()
+        n0 = ops.LAUNCHES[0]
+        with torch.cuda.graph(graph):
+            fc1 = run()
+        launches = ops.LAUNCHES[0] - n0
+
+        def replay():
+            graph.replay()
+            ops.LAUNCHES[0] += launches
+            return fc1
+        return replay
+
+    def head(self, fc1: torch.Tensor, prev_pose: torch.Tensor, next_pose: torch.Tensor) -> None:
+        """fc2 / fc3 / pose_norm of fc1 -> self.motion, and next_pose (7,) float64 = prev_pose (7,) float64 @ Exp(motion)"""
+        ops.posenet_head(fc1, self.net.head_blob, prev_pose, self.motion, next_pose)
+
+    @staticmethod
+    def _tensor(pose) -> torch.Tensor:
+        return (pose.tensor() if hasattr(pose, "ltype") else pose).reshape(-1)[:7]
+
+    def _wrap(self, pose: torch.Tensor):
+        return _pp.SE3(pose) if _pp is not None else pose
+
+    @torch.inference_mode()
+    def predict(self, frame, flow: torch.Tensor | None, depth: torch.Tensor | None):
+        if self.prev_pose is None:
+            self.prev_pose = torch.tensor([0., 0., 0., 0., 0., 0., 1.], device=self.device)
+            return self._wrap(self.prev_pose.clone())
+        assert flow is not None and depth is not None, "Motion model requires flow and depth to predict motion"
+        fc1 = self.enqueue(frame, flow, depth)
+        nxt = torch.empty((7,), dtype=torch.float64, device=self.device)
+        self.head(fc1, self.prev_pose.double(), nxt)
+        self.prev_pose = nxt.float()
+        return self._wrap(self.prev_pose.clone())
+
+    def update(self, pose) -> None:
+        self.prev_pose = self._tensor(pose).detach().to(device=self.device, dtype=torch.float32)
+
+    @classmethod
+    def is_valid_config(cls, config: SimpleNamespace | None) -> None:
+        cls._enforce_config_spec(config, {
+            "weight": lambda f: isinstance(f, str),
+            "device": lambda dev: isinstance(dev, str) and "cuda" in dev,
+        })
+
+
 PLUGINS = {
     "frontend": B200_FlowFormerCovFrontend,
     "keypoint": B200_CovAwareSelector_NoDepth,
@@ -569,4 +686,5 @@ PLUGINS = {
     "outlier": B200_CovarianceSanityFilter,
     "postprocess": B200_MotionInterpolate,
     "optimizer": B200_TwoFrame_PGO,
+    "motion": B200_TartanMotionNet,
 }
