@@ -400,7 +400,10 @@ int macvo_query_prep(const float* query, const float* ln_weight, const float* ln
  *   [0,3c) pos_Tw | [3c,5c) pixel2_uv | [5c,6c) pixel2_disp | [6c,9c) pixel2_uv_cov | [9c,10c) pixel2_disp_cov
  *   [10c,19c) obs1_covTc | [19c,28c) obs2_covTc | [28c,30c) pixel1_uv | [30c,31c) pixel1_d | [31c,31c+4) n_obs, n_inbound, k, status
  * (the first five sections are exactly the arrays macvo_pgo_solve_counted reads). *n_obs = survivors (device int).
- * *status (zeroed by the caller): 1 = a covariance patch left the image (the reference raises IndexError).
+ * *status (zeroed by the caller) is a bitmask, OR-ed by every observation that meets a condition:
+ *   bit 0 (1): a covariance patch crossed the bottom or right image edge (the reference raises IndexError; those
+ *              rows' covariances are unspecified). Patches crossing the top / left edge wrap like python indices.
+ *   bit 1 (2): a keypoint kp0 lies outside the image; its row is dropped and not counted in n_inbound.
  */
 /* CovarianceSanityFilter.filter (Module/OutlierFilter.py:91-100) on device-resident (k,3,3) float64 covariances:
  * good[i] = 1 iff neither matrix of observation i holds a NaN / Inf. */

@@ -59,7 +59,7 @@ observe_kernel(ObserveArgs A, float* __restrict__ rec, int* __restrict__ status)
     float* r = rec + (long long)i * REC;
     const bool in0 = u0 >= 0 && u0 < A.w && v0 >= 0 && v0 < A.h;
     if (!in0) {                                  // cannot happen for selector output; keep the table defined
-        if (lane == 0) { r[0] = 0.f; r[24] = 0.f; atomicExch(status, 2); }
+        if (lane == 0) { r[0] = 0.f; r[24] = 0.f; atomicOr(status, 2); }
         return;
     }
     const int p0 = (int)(v0 * A.w + u0);
@@ -87,7 +87,7 @@ observe_kernel(ObserveArgs A, float* __restrict__ rec, int* __restrict__ status)
     const float suv = A.match_cov[2 * hw + p0];
     oob |= macvo::match_cov_warp(u1, v1, ul1, vl1, A.depth1, A.h, A.w, suu, svv, suv, false, 0.f, A.P1, lane, c1);
     if (lane != 0) return;
-    if (oob) atomicExch(status, 1);
+    if (oob) atomicOr(status, 1);                // status is a bitmask: both conditions may occur in one call
     // CovarianceSanityFilter: drop observations with NaN / Inf covariance on either frame
     const bool keep = !(bad6(c0) || bad6(c1));
     // pixel2point_NED (Utility/Point.py:15-17): [d, (u - cx) / fx * d, (v - cy) / fy * d]
