@@ -273,6 +273,13 @@ int macvo_layer_norm(const float* x, const float* weight, const float* bias, flo
 /* sum_out = x + resid; y = LayerNorm(sum_out) in one pass (channels in {128, 256, 512}); sum_out may alias x or resid. */
 int macvo_add_layer_norm(const float* x, const float* resid, const float* weight, const float* bias, float* sum_out,
                          float* y, long long rows, int channels, float eps, void* stream);
+/* Transformer MLP with residual, TF32 tensor cores (sm_90a): out = resid + w2 GELU_erf(w1 xn + b1) + b2, row-wise.
+ * xn, resid, out (rows, channels) contiguous; w1 (hidden, channels), b1 (hidden), w2 (channels, hidden), b2 (channels);
+ * channels == 128, hidden in {128, 512} (else MACVO_E_UNSUPPORTED); every pointer 16-byte aligned; out may not alias xn.
+ * xn and the hidden activation (which never leaves the SM) are rounded to tf32, nearest-even, as cuBLAS rounds TF32 GEMM
+ * operands; w1 / w2 are truncated by the MMA, so pass them pre-rounded the same way to compute what cuBLAS TF32 computes. */
+int macvo_mlp_tc(const float* xn, const float* resid, const float* w1, const float* b1, const float* w2, const float* b2,
+                 float* out, int rows, int channels, int hidden, void* stream);
 /* maps (n_maps, 1, h, w) -> out (n_maps, ho, wo, 16) [NHWC], ho = ceil8(h)/2, wo = ceil8(w)/2:
  * ReLU(conv2d(zero-pad to multiples of 8, weight (16,1,6,6), stride 2, padding 2) + bias).
  * allow_tf32 bit 0: TF32 tensor-core implicit GEMM (what cuDNN does for the reference under cudnn.allow_tf32), else fp32 FMA.

@@ -20,6 +20,9 @@ static inline cudaStream_t as_stream(void* s) { return reinterpret_cast<cudaStre
 
 __host__ __device__ static inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 
+// exact (erf) GELU, the default of torch.nn.functional.gelu
+__device__ __forceinline__ static float gelu_erf(float x) { return 0.5f * x * (1.f + erff(x * 0.70710678118654752440f)); }
+
 template <typename T>
 __device__ __forceinline__ T warp_sum(T v) {
 #pragma unroll

@@ -39,8 +39,6 @@ template <int TP> struct Lay {
     static_assert(S_END * 4 <= 227 * 1024, "shared memory budget");
 };
 
-__device__ __forceinline__ float gelu_erf(float x) { return 0.5f * x * (1.f + erff(x * 0.70710678118654752440f)); }
-
 // acc[o][p] += sum_k WT[k][4 og + o] * X[k][4 pg + p]
 template <int K, int LD>
 __device__ __forceinline__ void gemm_tile(const float* __restrict__ WT, const float* __restrict__ X, int og, int pg,

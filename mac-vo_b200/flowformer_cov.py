@@ -251,6 +251,8 @@ class FlowFormerCovNet:
         self.gru_tensor_cores = os.environ.get("MACVO_B200_GRU_TC", "1") != "0"
         self.conv_tensor_cores = os.environ.get("MACVO_B200_CONV_TC", "1") != "0"      # same, the decoder's 3x3 / 1x1 convolutions
         self.gru_split_units = os.environ.get("MACVO_B200_GRU_SPLIT", "1") != "0"      # one launch chain per GRU unit on two streams
+        # TF32 mode only: the 128-channel transformer MLPs as one fused kernel (MACVO_B200_MLP_TC=0: cuBLAS GEMMs + GELU + add)
+        self.mlp_tensor_cores = os.environ.get("MACVO_B200_MLP_TC", "1") != "0"
         self._ops = None
         self._fused_conv_relu = True
         if corr_fn is None or lookup_fn is None or self.device.type == "cuda":
@@ -380,19 +382,26 @@ class FlowFormerCovNet:
             b0, b1 = p + f"blocks.{s}.0.", p + f"blocks.{s}.1."
             # block 0: locally-grouped attention (7x7 windows, zero padded after the norm)
             x, xn = self._add_ln(x, self._svt_local_attn(self._ln(x, b0 + "norm1", 1e-6), (H, W), b0 + "attn.", heads), b0 + "norm2", 1e-6)
-            x = x + self._mlp(xn, b0 + "mlp.")
+            x = self._mlp_residual(x, xn, b0 + "mlp.", "fc1", "fc2")
             # PEG: depthwise 3x3 + identity
             t = x.transpose(1, 2).reshape(B, C, H, W)          # channels-last view of the token matrix
             t = self._conv(t, p + f"pos_block.{s}.proj.0", padding=1, groups=C) + t
             x = t.flatten(2).transpose(1, 2)
             # block 1: globally sub-sampled attention
             x, xn = self._add_ln(x, self._svt_global_attn(self._ln(x, b1 + "norm1", 1e-6), (H, W), b1 + "attn.", heads, sr), b1 + "norm2", 1e-6)
-            x = x + self._mlp(xn, b1 + "mlp.")
+            x = self._mlp_residual(x, xn, b1 + "mlp.", "fc1", "fc2")
             x = x.reshape(B, H, W, C).permute(0, 3, 1, 2)      # (B, C, H, W) logical, channels-last in memory
         return x
 
-    def _mlp(self, x: Tensor, p: str) -> Tensor:
-        return self._lin(F.gelu(self._lin(x, p + "fc1")), p + "fc2")
+    def _mlp_residual(self, x: Tensor, xn: Tensor, p: str, fc1: str, fc2: str) -> Tensor:
+        """x + fc2(GELU(fc1(xn))); in TF32 mode at 128 channels one kernel (csrc/mlp_tc.cu) that keeps the hidden activation on
+        chip, with its weights rounded to tf32 once"""
+        w1 = self.W[p + fc1 + ".weight"]
+        if (self.mlp_tensor_cores and self._native(x) and torch.backends.cuda.matmul.allow_tf32 and x.shape[-1] == 128
+                and w1.shape[0] in self._ops.MLP_TC_HIDDEN and x.is_contiguous() and xn.is_contiguous()):
+            w1t, w2t = self._memo(("mlp_tc", p), lambda: (self._ops.round_tf32(w1), self._ops.round_tf32(self.W[p + fc2 + ".weight"])))
+            return self._ops.mlp_tc(xn, x, w1t, self.W[p + fc1 + ".bias"], w2t, self.W[p + fc2 + ".bias"])
+        return x + self._lin(F.gelu(self._lin(xn, p + fc1)), p + fc2)
 
     @staticmethod
     def _to_windows(x: Tensor, ws: int) -> tuple[Tensor, tuple[int, int, int, int]]:
@@ -478,7 +487,7 @@ class FlowFormerCovNet:
         y = self._ln(x, p + "norm1")
         a = self._attn(self._lin(y, p + "q"), self._lin(y, p + "k"), self._lin(y, p + "v"), 8)
         x, xn = self._add_ln(x, self._lin(a, p + "proj"), p + "norm2")
-        return x + self._lin(F.gelu(self._lin(xn, p + "ffn.0")), p + "ffn.3")
+        return self._mlp_residual(x, xn, p, "ffn.0", "ffn.3")
 
     def _context_tokens(self, context: Tensor, p: str, reps: int) -> Tensor:
         """context_proj of the context map, tiled like `context.repeat(B//b, 1, 1, 1)` (twins.py:55-58):
@@ -585,7 +594,7 @@ class FlowFormerCovNet:
     def _vert_block(self, x: Tensor, size, context: Tensor, p: str, local: bool) -> Tensor:
         attn = self._vert_local_attn if local else self._vert_global_attn
         x, xn = self._add_ln(x, attn(self._ln(x, p + "norm1"), size, context, p + "attn."), p + "norm2")
-        return x + self._mlp(xn, p + "mlp.")
+        return self._mlp_residual(x, xn, p + "mlp.", "fc1", "fc2")
 
     def cost_perceiver(self, cost_volume: Tensor, context: Tensor) -> tuple[Tensor, Tensor]:
         c = "memory_encoder.cost_perceiver_encoder."
@@ -604,7 +613,7 @@ class FlowFormerCovNet:
         else:
             a = self._attn(q, self._lin(tokens, p + "k"), self._lin(tokens, p + "v"), 8)
         x = lat + self._lin(a, p + "proj")
-        x = x + self._lin(F.gelu(self._lin(self._ln(x, p + "norm2"), p + "ffn.0")), p + "ffn.3")
+        x = self._mlp_residual(x, self._ln(x, p + "norm2"), p, "ffn.0", "ffn.3")
         short_cut = x
         N = H1 * W1
         self._join_context()                                      # first use of the context map

@@ -87,6 +87,7 @@ EXPORTS = {
                              + [C.c_void_p] * 2),
     "macvo_layer_norm": (C.c_int, [C.c_void_p] * 4 + [C.c_longlong, C.c_int, C.c_float, C.c_void_p]),
     "macvo_add_layer_norm": (C.c_int, [C.c_void_p] * 6 + [C.c_longlong, C.c_int, C.c_float, C.c_void_p]),
+    "macvo_mlp_tc": (C.c_int, [C.c_void_p] * 7 + [C.c_int] * 3 + [C.c_void_p]),
     "macvo_patch_embed_conv1": (C.c_int, [C.c_void_p] * 4 + [C.c_longlong, C.c_int, C.c_int, C.c_int, C.c_void_p]),
     "macvo_add_rows_relu": (C.c_int, [C.c_void_p] * 2 + [C.c_longlong, C.c_int, C.c_int, C.c_void_p]),
     "macvo_small_attention": (C.c_int, [C.c_void_p] * 4 + [C.c_int] * 7 + [C.c_void_p]),
@@ -787,6 +788,36 @@ def add_layer_norm(x: Tensor, resid: Tensor, weight: Tensor, bias: Tensor, eps: 
     _check(rc, "macvo_add_layer_norm")
     LAUNCHES[0] += 1
     return s, y
+
+
+MLP_TC_HIDDEN = (128, 512)
+
+
+def round_tf32(w: Tensor) -> Tensor:
+    """fp32 -> the nearest tf32 value (ties to even, like cvt.rn and like cuBLAS's TF32 GEMMs round their operands), still
+    stored as fp32: an MLP weight packed once for `mlp_tc`, whose tensor cores would otherwise truncate the low 13 mantissa
+    bits."""
+    i = w.detach().to(torch.float32).contiguous().view(torch.int32)
+    return ((i + 0xFFF + ((i >> 13) & 1)) & -0x2000).view(torch.float32)
+
+
+def mlp_tc(xn: Tensor, resid: Tensor, w1: Tensor, b1: Tensor, w2: Tensor, b2: Tensor) -> Tensor:
+    """resid + w2 GELU_erf(w1 xn + b1) + b2 over the last dim (128 channels, hidden size in MLP_TC_HIDDEN) in one TF32
+    tensor-core kernel (csrc/mlp_tc.cu); the hidden activation never reaches device memory."""
+    xn, resid = _dev(xn, torch.float32, "mlp_tc xn"), _dev(resid, torch.float32, "mlp_tc resid")
+    w1, w2 = _dev(w1, torch.float32, "mlp_tc w1"), _dev(w2, torch.float32, "mlp_tc w2")
+    b1, b2 = _dev(b1, torch.float32, "mlp_tc b1"), _dev(b2, torch.float32, "mlp_tc b2")
+    c, hd = xn.shape[-1], w1.shape[0]
+    if (c != 128 or hd not in MLP_TC_HIDDEN or xn.shape != resid.shape or tuple(w1.shape) != (hd, c)
+            or tuple(w2.shape) != (c, hd) or b1.numel() != hd or b2.numel() != c):
+        raise MacvoB200Error(f"mlp_tc: unsupported shapes xn {tuple(xn.shape)}, resid {tuple(resid.shape)}, "
+                             f"w1 {tuple(w1.shape)}, w2 {tuple(w2.shape)}")
+    out = torch.empty_like(resid)
+    rc = load_library().macvo_mlp_tc(xn.data_ptr(), resid.data_ptr(), w1.data_ptr(), b1.data_ptr(), w2.data_ptr(),
+                                      b2.data_ptr(), out.data_ptr(), xn.numel() // c, c, hd, _stream())
+    _check(rc, "macvo_mlp_tc")
+    LAUNCHES[0] += 1
+    return out
 
 
 def patch_embed_conv1(maps: Tensor, weight: Tensor, bias: Tensor, allow_tf32: bool | None = None, s2d: bool = False) -> Tensor:
