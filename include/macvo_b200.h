@@ -342,11 +342,6 @@ int macvo_gru_blend(const float* q, const float* bias, const float* z, float* hx
  *             which the result is ADDED in place (the decoder's `coords1 = coords1 + delta_flow`, covhead.py:133-134).
  *             Only columns n < n_valid are stored. */
 size_t macvo_rows_count(int batch, int height, int width, int vertical);
-/* profiling aid: device buffer of 1 + 3 * capacity uint64 = event count, then (kernel id, start ns, end ns) per launch of the
- * tensor-core convolution / GRU kernels; NULL (the default) switches it off */
-void macvo_tc_set_timeline(void* buf, int capacity);
-/* profiling aid: 3 x 64 uint64 globaltimer events (producer | MMA steps | epilogue) of block (0,0) of macvo_conv_tc; NULL = off */
-void macvo_conv_tc_set_trace(void* buf);
 int macvo_conv_tc(const void* in_rows, int in_channels, int in_dense, const void* weights, const float* bias, int n_pad,
                   int n_valid, int ksize, int relu, int batch, int height, int width, void* out16, int out16_pitch,
                   int out16_offset, int out16_dense, float* out32, int out32_pitch, int out32_offset, int out32_planes,
@@ -358,22 +353,19 @@ int macvo_flow_im2col(const float* coords1, const float* coords0, void* rows, fl
                       int height, int width, void* stream);
 
 /* ---- SepConvGRU on wgmma (csrc/gru_conv_tc.cu): the 1x5 / 5x1 gate convolutions of gru.py:22-43 as implicit GEMMs with the
- * gate math in the epilogue, for `units` (1 or 2: flow, covariance — covhead.py:95-131) recurrent units per launch.
+ * gate math in the epilogue, for one recurrent unit (flow or covariance — covhead.py:95-131) per launch.
  * Operands are fp16 PADDED pixel rows: pass `vertical` = 0 (1x5) uses layout U (above), `vertical` = 1 (5x1) stores pixel
  * (b, y, x) at row 2 + (b W + x)(H + 4) + y + 2; all other rows must be zero (allocate
  * macvo_gru_tc_operand_rows(...) zeroed rows once; the kernels only ever write pixel rows).
- *   h_rows[u]   (rows, 128) fp16: stage 0: h, stage 1: r*h          x_rows (rows, 384) fp16: [inp | mf | mf + gamma agg]
- *   weights[u]  (N, 5*512) fp16, K index = tap * 512 + channel of cat[h, x]; N = 256 (z | r) for stage 0, 128 (q) for stage 1
- *   bias[u] (N) fp32;  h_master[u], z[u] (pixels, 128) fp32 in dense pixel order (the recurrent state stays fp32)
- *   out_rows[u] (rows', 128) fp16: stage 0 writes r*h rows of THIS pass's layout, stage 1 writes the new h in the OTHER
+ *   h_rows      (rows, 128) fp16: stage 0: h, stage 1: r*h          x_rows (rows, 384) fp16: [inp | mf | mf + gamma agg]
+ *   weights     (N, 5*512) fp16, K index = tap * 512 + channel of cat[h, x]; N = 256 (z | r) for stage 0, 128 (q) for stage 1
+ *   bias (N) fp32;  h_master, z (pixels, 128) fp32 in dense pixel order (the recurrent state stays fp32)
+ *   out_rows    (rows', 128) fp16: stage 0 writes r*h rows of THIS pass's layout, stage 1 writes the new h in the OTHER
  *   pass's layout (the next pass's input) and updates h_master in place.
  * stage 0: z = sigmoid(conv + b)[:128] -> z;  r*h -> out_rows.     stage 1: h <- (1 - z) h + z tanh(conv + b). */
 size_t macvo_gru_tc_operand_rows(int batch, int height, int width, int vertical);
-int macvo_gru_tc_stage(int stage, int vertical, int batch, int height, int width, int units, const void* const* h_rows,
-                       const void* x_rows, const void* const* weights, const float* const* bias, float* const* h_master,
-                       float* const* z, void* const* out_rows, void* stream);
-/* profiling aid: device buffer of 3 x 64 uint64 that the first CTA fills with globaltimer events (NULL = off, the default) */
-void macvo_gru_tc_set_trace(void* buf);
+int macvo_gru_tc_stage(int stage, int vertical, int batch, int height, int width, const void* h_rows, const void* x_rows,
+                       const void* weights, const float* bias, float* h_master, float* z, void* out_rows, void* stream);
 /* fp32 dense pixel rows src (pixels, src_pitch)[:, :channels] -> fp16 operand rows dst[:, dst_offset : dst_offset + channels] */
 int macvo_gru_tc_pack(const float* src, int src_pitch, int channels, void* dst, int dst_channels, int dst_offset, int batch,
                       int height, int width, int vertical, void* stream);
@@ -389,10 +381,6 @@ int macvo_softmax_rows_f16(const float* scores, void* out, long long rows, int c
  * out[n, c, 8y+i, 8x+j] = sum_k softmax_k(scale * mask[.., k*64 + i*8 + j]) * 8 * flow[n, c, y + k/3 - 1, x + k%3 - 1] (zero outside) */
 int macvo_convex_upsample(const float* flow, const float* mask_nhwc, float* out, float scale, int batch, int height, int width,
                           void* stream);
-/* out (pixels,64) = LayerNorm_64(query) + LinearPositionEmbeddingSine(coords)  (decoder.py:56-66, attention.py:71-101);
- * coords (batch, 2, n1) [x, y]; freq: the 16 fp32 frequencies k*pi/200. */
-int macvo_query_prep(const float* query, const float* ln_weight, const float* ln_bias, const float* coords,
-                     const float* freq, float* out, int batch, int n1, float eps, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * (f3) observation building + sanity filter + MatchObs packing on the device — replaces the host code of

@@ -34,8 +34,6 @@ struct ConvArgs {
     __half* out16; int out16_pitch, out16_off, out16_dense;
     float* out32; int out32_pitch, out32_off;
     int out32_planes;             // 1: out32 is a (batch, n_valid, H, W) map and the result is ADDED to it (coords += delta)
-    Timeline tl;                  // profiling aid, buf == NULL in production
-    unsigned long long* trace;    // profiling aid: [role][64] globaltimer events of block (0, 0)
 };
 
 // N = output channels per CTA (multiple of 32, <= 256); grid.y slices the padded output channels
@@ -50,17 +48,6 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int tile = blockIdx.x, slice = blockIdx.y;
-    Timeline tl = a.tl;
-    tl.begin(100 + a.taps * 1000 + a.kblocks * 10000 + N * 100000);
-    int tr_n = 0;
-    auto TR = [&](int role) {
-        if (a.trace != nullptr && blockIdx.x == 0 && blockIdx.y == 0 && tr_n < 64) {
-            unsigned long long t;
-            asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-            a.trace[role * 64 + tr_n++] = t;
-        }
-    };
-    if (warp == 0 && lane == 0) TR(2);
     const int steps = a.kblocks * a.taps;
 
     if (threadIdx.x == 0) {
@@ -91,7 +78,6 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
             const int pre = steps < a.slots ? steps : a.slots;
             { int k2 = 0, t2 = 0; for (int g = 0; g < pre; ++g) { issue_w(g, k2, t2); advance(k2, t2); } }
             asm volatile("griddepcontrol.wait;" ::: "memory");
-            TR(0);
             int slot = 0, kb = 0, tap = 0;
             uint32_t phase = 0;
             for (int g = 0; g < steps; ++g) {
@@ -100,7 +86,6 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
                     issue_w(slot, kb, tap);
                 }
                 issue_a(slot, kb, tap);
-                TR(0);
                 advance(kb, tap);
                 if (++slot == a.slots) { slot = 0; phase ^= 1; }
             }
@@ -115,7 +100,6 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
         int slot = 0, prev = 0; uint32_t phase = 0;
         for (int g = 0; g < steps; ++g) {
             mbar_wait(bar_full + 8 * slot, phase);
-            if (warp == 0 && lane == 0) TR(1);
             const uint32_t sa = smem_u32(smem + slot * SLOT_BYTES);
             const uint64_t da = make_kmajor_sw128_desc(sa + wg * 64 * 128), db = make_kmajor_sw128_desc(sa + A_BYTES);
             wgmma_fence();
@@ -162,7 +146,6 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
     const uint32_t stage_q = smem_u32(smem) + quarter * 32 * pitch;
     asm volatile("griddepcontrol.wait;" ::: "memory");            // nothing of the previous kernel is overwritten before it finished
     consumers_sync();                                              // all rows staged
-    if (warp == 0 && lane == 0) TR(2);
     // (every lane runs every iteration — the shuffles below need the whole warp; lanes past the slice only skip the stores)
     for (int cg = 0; cg * 128 < N; ++cg) {
         const int col = cg * 128 + 4 * lane, gcol = slice * N + col;
@@ -198,8 +181,6 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
             }
         }
     }
-    if (threadIdx.x == 0) tl.end();
-    if (warp == 0 && lane == 0) TR(2);
 }
 
 // 7x7 neighbourhood of the 2-channel flow as GEMM rows (the motion encoder's convf1, gru.py:50,57, becomes a 1x1 convolution):
@@ -260,13 +241,6 @@ int launch_conv(const CUtensorMap& map_a, const CUtensorMap& map_w, const ConvAr
 
 }  // namespace
 
-static Timeline g_timeline = {nullptr, 0, -1};
-static unsigned long long* g_conv_trace = nullptr;
-extern "C" void macvo_conv_tc_set_trace(void* buf) { g_conv_trace = static_cast<unsigned long long*>(buf); }
-/* profiling aid (tools/decoder_timeline.py): device buffer of 1 + 3 * capacity uint64; NULL switches it off (the default) */
-extern "C" void macvo_tc_set_timeline(void* buf, int capacity) { g_timeline.buf = static_cast<unsigned long long*>(buf); g_timeline.capacity = capacity; }
-Timeline macvo_tc_timeline() { return g_timeline; }
-
 extern "C" size_t macvo_rows_count(int batch, int height, int width, int vertical) {
     if (batch <= 0 || height <= 0 || width <= 0) return 0;
     return (size_t)macvo_rows::alloc_rows(batch, height, width, vertical);
@@ -304,8 +278,6 @@ extern "C" int macvo_conv_tc(const void* in_rows, int in_channels, int in_dense,
     a.relu = relu; a.n_valid = n_valid; a.bias = bias;
     a.out16 = static_cast<__half*>(out16); a.out16_pitch = out16_pitch; a.out16_off = out16_offset; a.out16_dense = out16_dense;
     a.out32 = out32; a.out32_pitch = out32_pitch; a.out32_off = out32_offset; a.out32_planes = out32_planes;
-    a.tl = g_timeline;
-    a.trace = g_conv_trace;
     CUtensorMap map_a, map_w;
     const uint64_t in_rows_total = in_dense ? (uint64_t)a.m_rows : (uint64_t)macvo_rows::alloc_rows(batch, height, width, 0);
     if (!make_map_2d(&map_a, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, in_rows, in_channels, in_rows_total, (uint64_t)in_channels * 2, BLOCK_K, TILE_M))

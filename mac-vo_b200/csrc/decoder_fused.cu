@@ -85,31 +85,6 @@ gru_blend_kernel(const float* __restrict__ q, const float* __restrict__ bias, co
     if (h_dense) *reinterpret_cast<float4*>(h_dense + p * HID + c) = o;
 }
 
-// q_in = LayerNorm(query) + sine_embed(coords1): the input of the cross-attention query projection
-// (decoder.py:56-66, attention.py:71-101 LinearPositionEmbeddingSine with dim 64: [sin x f | cos x f | sin y f | cos y f],
-// f = k * pi / 200, k = 0..15 — passed in as the fp32 table torch builds). One warp per pixel, two channels per lane.
-__global__ void __launch_bounds__(256)
-query_prep_kernel(const float* __restrict__ query, const float* __restrict__ w, const float* __restrict__ b,
-                  const float* __restrict__ coords, const float* __restrict__ freq, float* __restrict__ out,
-                  long long pixels, int n1, float eps) {
-    const long long p = (long long)blockIdx.x * 8 + (threadIdx.x >> 5);
-    const int lane = threadIdx.x & 31;
-    if (p >= pixels) return;
-    const float2 t = *reinterpret_cast<const float2*>(query + p * 64 + lane * 2);
-    const float mean = warp_sum(t.x + t.y) * (1.f / 64);
-    const float d0 = t.x - mean, d1 = t.y - mean;
-    const float rstd = rsqrtf(warp_sum(fmaf(d0, d0, d1 * d1)) * (1.f / 64) + eps);
-    const float2 ww = *reinterpret_cast<const float2*>(w + lane * 2), bb = *reinterpret_cast<const float2*>(b + lane * 2);
-    const long long bi = p / n1, pi = p % n1;
-    const int grp = lane >> 3;                                   // channels 2*lane, 2*lane+1 -> group of 16
-    const float c = coords[(bi * 2 + (grp >> 1)) * n1 + pi];     // groups 0,1 use x; 2,3 use y
-    const int k = (2 * lane) & 15;
-    const float a0 = __fmul_rn(c, freq[k]), a1 = __fmul_rn(c, freq[k + 1]);
-    const float e0 = (grp & 1) ? cosf(a0) : sinf(a0), e1 = (grp & 1) ? cosf(a1) : sinf(a1);
-    *reinterpret_cast<float2*>(out + p * 64 + lane * 2) =
-        make_float2(__fadd_rn(d0 * rstd * ww.x + bb.x, e0), __fadd_rn(d1 * rstd * ww.y + bb.y, e1));
-}
-
 inline unsigned grid_for(long long pixels) { return (unsigned)((pixels * (HID / 4) + 255) / 256); }
 
 }  // namespace
@@ -137,16 +112,6 @@ extern "C" int macvo_gru_blend(const float* q, const float* bias, const float* z
     if (!q || !z || !hx || pixels < 0) return MACVO_E_ARG;
     if (pixels == 0) return MACVO_OK;
     gru_blend_kernel<<<grid_for(pixels), 256, 0, as_stream(stream)>>>(q, bias, z, hx, h_dense, pixels);
-    MACVO_LAUNCH_CHECK();
-    return MACVO_OK;
-}
-
-extern "C" int macvo_query_prep(const float* query, const float* ln_weight, const float* ln_bias, const float* coords,
-                                const float* freq, float* out, int batch, int n1, float eps, void* stream) {
-    if (!query || !ln_weight || !ln_bias || !coords || !freq || !out || batch <= 0 || n1 <= 0) return MACVO_E_ARG;
-    const long long pixels = (long long)batch * n1;
-    query_prep_kernel<<<(unsigned)((pixels + 7) / 8), 256, 0, as_stream(stream)>>>(query, ln_weight, ln_bias, coords, freq,
-                                                                                   out, pixels, n1, eps);
     MACVO_LAUNCH_CHECK();
     return MACVO_OK;
 }

@@ -2,7 +2,7 @@
 // (flow + covariance) as implicit GEMMs with the gate math in the epilogue. Replaces, per refinement iteration and pass,
 //   zr = conv(cat[h, x]) ; z, r = sigmoid(zr) ; q = tanh(conv(cat[r*h, x])) ; h = (1-z) h + z q
 // (Module/Network/FlowFormer/core/gru.py:22-43, update blocks covhead.py:95-131) — 8 cuDNN convolutions + 8 glue launches per
-// iteration before, 4 launches now (stage 0: z|r of both units, stage 1: q + blend of both units, for each of the two passes).
+// unit and iteration before, 4 launches now (stage 0: z|r, stage 1: q + blend, for each of the two passes).
 //
 // GEMM view of one stage: rows = pixels (M), columns = output channels (N = 256 for z|r, 128 for q), K = 5 taps x 512
 // channels. Operands are fp16 (11-bit significand >= TF32's 10; the recurrent state itself stays fp32 in `h_master`, only
@@ -16,7 +16,7 @@
 // The x part of the input (384 of the 512 channels: context | motion features | aggregated motion) is identical for both
 // units and both stages: it lives in one buffer per layout; the h / r*h part is a separate 128-channel buffer per unit.
 //
-// One CTA per (unit, 128-pixel tile): warps 0..7 = two consumer warpgroups (m64nNk16 wgmma), warp 8 = TMA producer.
+// One launch per unit, one CTA per 128-pixel tile: warps 0..7 = two consumer warpgroups (m64nNk16 wgmma), warp 8 = TMA producer.
 #include "tc_common.cuh"
 #include "rows_layout.cuh"
 #include <cuda_fp16.h>
@@ -48,17 +48,14 @@ struct Unit {                    // one recurrent unit (flow / covariance)
 struct Geometry {
     int batch, height, width, vertical;
     int lines, len, lp;          // lines of `len` pixels, padded pitch lp = len + 4
-    int m_pad, tiles;            // padded pixels, 128-pixel tiles per unit
-    unsigned long long* trace;   // profiling aid (NULL in production): globaltimer events of the first CTA, [role][event]
-    Timeline tl;                 // profiling aid: in-stream timeline shared with csrc/conv_tc.cu
+    int m_pad, tiles;            // padded pixels, 128-pixel tiles
 };
 
 // STAGE 0: N = 256 (z | r)   STAGE 1: N = 128 (q, then the blend)
 template <int STAGE>
 __global__ void __launch_bounds__(TC_THREADS, 1)
-gru_conv_tc_kernel(const __grid_constant__ CUtensorMap map_h0, const __grid_constant__ CUtensorMap map_h1,
-                   const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_w0,
-                   const __grid_constant__ CUtensorMap map_w1, Unit u0, Unit u1, Geometry g) {
+gru_conv_tc_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant__ CUtensorMap map_x,
+                   const __grid_constant__ CUtensorMap map_w, Unit u, Geometry g) {
     constexpr int N = STAGE == 0 ? 256 : 128;
     using C = Cfg<N>;
     extern __shared__ uint8_t smem_raw[];
@@ -66,25 +63,12 @@ gru_conv_tc_kernel(const __grid_constant__ CUtensorMap map_h0, const __grid_cons
     const uint32_t bar_full = smem_u32(smem + C::SLOTS * C::SLOT_BYTES), bar_empty = bar_full + 8 * C::SLOTS;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int unit = blockIdx.x / g.tiles, tile = blockIdx.x - unit * g.tiles;   // this CTA's 128 padded pixels
-    const Unit u = unit == 0 ? u0 : u1;
-    const CUtensorMap* map_h = unit == 0 ? &map_h0 : &map_h1;
-    const CUtensorMap* map_w = unit == 0 ? &map_w0 : &map_w1;
-    g.tl.begin(STAGE + 2 * g.vertical);
-    int tr_n = 0;
-    auto TR = [&](int role) {
-        if (g.trace != nullptr && blockIdx.x == 0 && tr_n < 64) {
-            unsigned long long t;
-            asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-            g.trace[role * 64 + tr_n++] = t;
-        }
-    };
-    if (warp == 0 && lane == 0) TR(2);
+    const int tile = blockIdx.x;                                          // this CTA's 128 padded pixels
 
     if (threadIdx.x == 0) {
         for (int s = 0; s < C::SLOTS; ++s) { mbar_init(bar_full + 8 * s, 1); mbar_init(bar_empty + 8 * s, 2); }
         fence_barrier_init();
-        prefetch_tmap(map_h); prefetch_tmap(&map_x); prefetch_tmap(map_w);
+        prefetch_tmap(&map_h); prefetch_tmap(&map_x); prefetch_tmap(&map_w);
     }
     __syncthreads();
     // Programmatic dependent launch: the next stage may start as soon as every CTA of this one got here. Its weights and the x
@@ -96,18 +80,16 @@ gru_conv_tc_kernel(const __grid_constant__ CUtensorMap map_h0, const __grid_cons
         // ===================== TMA producer =====================
         if (elect_one()) {
             int slot = 0; uint32_t phase = 0;
-            TR(0);
             for (int it = 0; it < KBLOCKS; ++it) {
                 const int kb = (it + HID / BLOCK_K) % KBLOCKS;                 // 2, 3, ..., 7, 0, 1
                 if (kb == 0) asm volatile("griddepcontrol.wait;" ::: "memory");
                 for (int t = 0; t < TAPS; ++t) {
                     mbar_wait(bar_empty + 8 * slot, phase ^ 1);
-                    TR(0);
                     const uint32_t full = bar_full + 8 * slot, sa = smem_u32(smem + slot * C::SLOT_BYTES);
                     mbar_expect_tx(full, C::SLOT_BYTES);
-                    if (kb < HID / BLOCK_K) tma_load_2d(sa, map_h, full, kb * BLOCK_K, tile * TILE_M + t);
+                    if (kb < HID / BLOCK_K) tma_load_2d(sa, &map_h, full, kb * BLOCK_K, tile * TILE_M + t);
                     else tma_load_2d(sa, &map_x, full, kb * BLOCK_K - HID, tile * TILE_M + t);
-                    tma_load_2d(sa + A_BYTES, map_w, full, t * CIN + kb * BLOCK_K, 0);
+                    tma_load_2d(sa + A_BYTES, &map_w, full, t * CIN + kb * BLOCK_K, 0);
                     if (++slot == C::SLOTS) { slot = 0; phase ^= 1; }
                 }
             }
@@ -122,7 +104,6 @@ gru_conv_tc_kernel(const __grid_constant__ CUtensorMap map_h0, const __grid_cons
         int slot = 0, prev = 0; uint32_t phase = 0;
         for (int s = 0; s < KBLOCKS * TAPS; ++s) {
             mbar_wait(bar_full + 8 * slot, phase);
-            if (warp == 0 && lane == 0) TR(1);
             const uint32_t sa = smem_u32(smem + slot * C::SLOT_BYTES);
             const uint64_t da = make_kmajor_sw128_desc(sa + wg * 64 * 128), db = make_kmajor_sw128_desc(sa + A_BYTES);
             wgmma_fence();
@@ -175,7 +156,6 @@ gru_conv_tc_kernel(const __grid_constant__ CUtensorMap map_h0, const __grid_cons
         }
     }
     consumers_sync();                                                     // all rows staged
-    if (warp == 0 && lane == 0) TR(2);
     if (STAGE == 0) {
         // half 0: z columns [0, 128) -> z buffer      half 1: r columns [128, 256) -> r * h operand rows (this layout)
         const float4 bb = __ldg(reinterpret_cast<const float4*>(u.bias + half * 128 + 4 * lane));
@@ -216,8 +196,6 @@ gru_conv_tc_kernel(const __grid_constant__ CUtensorMap map_h0, const __grid_cons
             *reinterpret_cast<uint2*>(u.out + orow * HID + 4 * lane) = *reinterpret_cast<uint2*>(h2);
         }
     }
-    if (warp == 0 && lane == 0) TR(2);
-    g.tl.end();
 }
 
 // fp32 pixel rows (dense order) -> fp16 operand rows of one layout (pad rows are never written: they stay zero)
@@ -267,8 +245,6 @@ Geometry make_geometry(int batch, int height, int width, int vertical) {
     g.lp = g.len + 4;
     g.m_pad = g.lines * g.lp;
     g.tiles = (g.m_pad + TILE_M - 1) / TILE_M;
-    g.trace = nullptr;
-    g.tl = Timeline{nullptr, 0, -1};
     return g;
 }
 size_t operand_rows(const Geometry& g) { return (size_t)macvo_rows::alloc_rows(g.batch, g.height, g.width, g.vertical); }
@@ -280,7 +256,7 @@ bool make_map_a(CUtensorMap* map, const void* base, int channels, const Geometry
 }
 
 template <int STAGE>
-int launch_stage(const CUtensorMap* maps, Unit u0, Unit u1, const Geometry& g, int units, cudaStream_t stream) {
+int launch_stage(const CUtensorMap* maps, Unit u, const Geometry& g, cudaStream_t stream) {
     constexpr int N = STAGE == 0 ? 256 : 128;
     static bool configured = false;
     if (!configured) {
@@ -288,7 +264,7 @@ int launch_stage(const CUtensorMap* maps, Unit u0, Unit u1, const Geometry& g, i
         configured = true;
     }
     cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(g.tiles * units);
+    cfg.gridDim = dim3(g.tiles);
     cfg.blockDim = dim3(TC_THREADS);
     cfg.dynamicSmemBytes = Cfg<N>::SMEM;
     cfg.stream = stream;
@@ -297,16 +273,11 @@ int launch_stage(const CUtensorMap* maps, Unit u0, Unit u1, const Geometry& g, i
     attrs[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attrs;
     cfg.numAttrs = 1;
-    MACVO_CUDA_TRY(cudaLaunchKernelEx(&cfg, gru_conv_tc_kernel<STAGE>, maps[0], maps[1], maps[2], maps[3], maps[4], u0, u1, g));
+    MACVO_CUDA_TRY(cudaLaunchKernelEx(&cfg, gru_conv_tc_kernel<STAGE>, maps[0], maps[1], maps[2], u, g));
     return MACVO_OK;
 }
 
 }  // namespace
-
-Timeline macvo_tc_timeline();          // csrc/conv_tc.cu
-static unsigned long long* g_trace = nullptr;
-/* profiling aid (tools/gru_probe.py): device buffer of 3 x 64 u64 that the first CTA fills with globaltimer events */
-extern "C" void macvo_gru_tc_set_trace(void* buf) { g_trace = static_cast<unsigned long long*>(buf); }
 
 extern "C" size_t macvo_gru_tc_operand_rows(int batch, int height, int width, int vertical) {
     if (batch <= 0 || height <= 0 || width <= 0) return 0;
@@ -337,32 +308,18 @@ extern "C" int macvo_gru_tc_pack_motion(const float* mf, const float* agg, const
     return MACVO_OK;
 }
 
-extern "C" int macvo_gru_tc_stage(int stage, int vertical, int batch, int height, int width, int units, const void* const* h_rows,
-                                  const void* x_rows, const void* const* weights, const float* const* bias, float* const* h_master,
-                                  float* const* z, void* const* out_rows, void* stream) {
-    if ((stage != 0 && stage != 1) || (units != 1 && units != 2) || batch <= 0 || height <= 0 || width <= 0 || !h_rows || !x_rows ||
-        !weights || !bias || !h_master || !z || !out_rows)
+extern "C" int macvo_gru_tc_stage(int stage, int vertical, int batch, int height, int width, const void* h_rows, const void* x_rows,
+                                  const void* weights, const float* bias, float* h_master, float* z, void* out_rows, void* stream) {
+    if ((stage != 0 && stage != 1) || batch <= 0 || height <= 0 || width <= 0 || !h_rows || !x_rows || !weights || !bias ||
+        !h_master || !z || !out_rows)
         return MACVO_E_ARG;
-    for (int i = 0; i < units; ++i)
-        if (!h_rows[i] || !weights[i] || !bias[i] || !h_master[i] || !z[i] || !out_rows[i]) return MACVO_E_ARG;
-    Geometry g = make_geometry(batch, height, width, vertical);
-    g.trace = g_trace;
-    g.tl = macvo_tc_timeline();
+    const Geometry g = make_geometry(batch, height, width, vertical);
     const int n = stage == 0 ? 256 : 128;
-    CUtensorMap maps[5];
-    for (int i = 0; i < 2; ++i) {
-        const int s = i < units ? i : 0;
-        if (!make_map_a(&maps[i], h_rows[s], HID, g)) return MACVO_E_UNSUPPORTED;
-        if (!make_map_2d(&maps[3 + i], CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, weights[s], (uint64_t)TAPS * CIN, n, (uint64_t)TAPS * CIN * 2,
-                         BLOCK_K, n))
-            return MACVO_E_UNSUPPORTED;
-    }
-    if (!make_map_a(&maps[2], x_rows, XCH, g)) return MACVO_E_UNSUPPORTED;
-    Unit u[2];
-    for (int i = 0; i < 2; ++i) {
-        const int s = i < units ? i : 0;
-        u[i].bias = bias[s]; u[i].h_master = h_master[s]; u[i].z = z[s]; u[i].out = static_cast<__half*>(out_rows[s]);
-    }
-    return stage == 0 ? launch_stage<0>(maps, u[0], u[1], g, units, as_stream(stream))
-                      : launch_stage<1>(maps, u[0], u[1], g, units, as_stream(stream));
+    CUtensorMap maps[3];                                                  // h | x | weights
+    if (!make_map_a(&maps[0], h_rows, HID, g) || !make_map_a(&maps[1], x_rows, XCH, g) ||
+        !make_map_2d(&maps[2], CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, weights, (uint64_t)TAPS * CIN, n, (uint64_t)TAPS * CIN * 2, BLOCK_K, n))
+        return MACVO_E_UNSUPPORTED;
+    Unit u;
+    u.bias = bias; u.h_master = h_master; u.z = z; u.out = static_cast<__half*>(out_rows);
+    return stage == 0 ? launch_stage<0>(maps, u, g, as_stream(stream)) : launch_stage<1>(maps, u, g, as_stream(stream));
 }

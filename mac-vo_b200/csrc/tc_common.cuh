@@ -118,32 +118,6 @@ __device__ __forceinline__ void stage_acc_rows(uint32_t base, int pitch, const f
     }
 }
 
-// ---- profiling aid: in-stream timeline (globaltimer) of the tensor-core kernels --------------------------------------------
-// buf[0] = event counter, then (kernel id, start ns, end ns) triples written by thread 0 of block 0 of every launch.
-struct Timeline {
-    unsigned long long* buf; int capacity, slot;
-    __device__ __forceinline__ void begin(int id) {
-        slot = -1;
-        if (buf != nullptr && blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0) {
-            const int i = (int)atomicAdd(buf, 1ULL);
-            if (i < capacity) {
-                slot = i;
-                unsigned long long t;
-                asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-                buf[1 + 3 * i] = (unsigned long long)id;
-                buf[2 + 3 * i] = t;
-            }
-        }
-    }
-    __device__ __forceinline__ void end() {
-        if (slot >= 0) {
-            unsigned long long t;
-            asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-            buf[3 + 3 * slot] = t;
-        }
-    }
-};
-
 // ---- host side: tensor maps ------------------------------------------------------------------------------------
 typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                     const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,

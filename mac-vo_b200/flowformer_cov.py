@@ -12,16 +12,16 @@ re-implementation of the reference network
 
 Plain GEMMs and convolutions go through torch (cuBLAS / cuDNN — library GEMMs); everything memory-bound on a CUDA
 fp32 run goes through our own kernels (`csrc/nn_kernels.cu`, `csrc/decoder_fused.cu`: LayerNorm, PatchEmbed conv1,
-the attention family incl. the K/V-free perceiver input layer, the SepConvGRU glue on NHWC `[h|x]` state buffers, the
-decoder's query preparation); CPU tensors and half-precision runs keep the torch ops (`_native()`), which is also how
-the class is checked against the reference network's golden outputs on the CPU. The two operators
-`BASELINE.json: north_star` names are NOT torch ops here:
+the attention family incl. the K/V-free perceiver input layer, the SepConvGRU glue on NHWC `[h|x]` state buffers); CPU
+tensors and half-precision runs keep the torch ops (`_native()`), which is also how the class is checked against the
+reference network's golden outputs on the CPU. The two operators `BASELINE.json: north_star` names are NOT torch ops here:
 
 * `corr_fn(f1, f2) -> (B, 1, H1, W1, H1, W1)`   all-pairs correlation volume (encoder.py:256-275)
 * `lookup_fn(cost_maps, coords) -> (B, 81, H1, W1)`  9x9 window lookup (decoder.py:141-153)
 
 By default both bind to the sm_90a CUDA kernels behind the C-ABI (`ops.corr_build`, `ops.corr_lookup`)
-and fail loudly when the library / a GPU is missing. Tests inject the CPU oracle instead.
+and fail loudly when the library / a GPU is missing. Tests inject the CPU oracle instead; a CUDA network always looks up
+with `ops.corr_lookup`.
 
 Restructuring relative to the reference (same arithmetic per output, fewer launches / bytes):
 * weights live in a flat dict keyed by the checkpoint names, the forward pass is functional;
@@ -247,16 +247,14 @@ class FlowFormerCovNet:
                  lookup_fn: Callable[[Tensor, Tensor], Tensor] | None = None):
         self.device = torch.device(device)
         self.enc_dtype, self.dec_dtype, self.depth = enc_dtype, dec_dtype, decoder_depth
-        # TF32 mode only: SepConvGRU on the tensor-core kernel (False / MACVO_B200_GRU_TC=0: cuDNN convolutions + glue kernels)
-        self.gru_tensor_cores = os.environ.get("MACVO_B200_GRU_TC", "1") != "0"
-        self.conv_tensor_cores = os.environ.get("MACVO_B200_CONV_TC", "1") != "0"      # same, the decoder's 3x3 / 1x1 convolutions
-        self.gru_split_units = os.environ.get("MACVO_B200_GRU_SPLIT", "1") != "0"      # one launch chain per GRU unit on two streams
         # TF32 mode only: the 128-channel transformer MLPs as one fused kernel (MACVO_B200_MLP_TC=0: cuBLAS GEMMs + GELU + add)
         self.mlp_tensor_cores = os.environ.get("MACVO_B200_MLP_TC", "1") != "0"
         self._ops = None
-        self._fused_conv_relu = True
         if corr_fn is None or lookup_fn is None or self.device.type == "cuda":
             from . import ops  # binds to the CUDA library; raises if it cannot be loaded
+            if self.device.type == "cuda" and lookup_fn is not None and lookup_fn is not ops.corr_lookup:
+                raise ValueError("a CUDA FlowFormerCovNet looks up with ops.corr_lookup (its decoder reads the lookup rows "
+                                 "directly); inject a lookup_fn only into a CPU network")
             corr_fn = corr_fn or ops.corr_build
             lookup_fn = lookup_fn or ops.corr_lookup
             self._ops = ops if self.device.type == "cuda" else None
@@ -325,7 +323,7 @@ class FlowFormerCovNet:
 
     def _conv_relu(self, x: Tensor, p: str, stride=1, padding=0) -> Tensor:
         """relu(conv2d(x) + bias): one cuDNN fused conv-bias-activation launch on the GPU path."""
-        if self._ops is not None and x.is_cuda and self._fused_conv_relu:
+        if self._ops is not None and x.is_cuda:
             if not x.is_contiguous(memory_format=torch.channels_last):
                 x = x.contiguous(memory_format=torch.channels_last)
             pair = lambda v: (v, v) if isinstance(v, int) else tuple(v)
@@ -443,7 +441,7 @@ class FlowFormerCovNet:
         p = "memory_encoder.cost_perceiver_encoder.patch_embed."
         M, _, H2, W2 = cost_maps.shape
         if self._native(cost_maps) and (H2 + 7) // 8 * 8 * ((W2 + 7) // 8 * 8) <= 96 * 160:
-            if torch.backends.cudnn.allow_tf32 and self._fused_conv_relu:
+            if torch.backends.cudnn.allow_tf32:
                 # conv1 written space-to-depth -> proj.2 (6x6 / s2 over 16 channels, half-empty K blocks in the implicit GEMM)
                 # runs as the equivalent 3x3 / s1 convolution over 64 channels
                 x = self._ops.patch_embed_conv1(cost_maps, self.W[p + "proj.0.weight"], self.W[p + "proj.0.bias"], s2d=True)
@@ -709,218 +707,49 @@ class FlowFormerCovNet:
         out = (mask.unsqueeze(1) * up.unsqueeze(-3).unsqueeze(-3)).sum(dim=2)
         return out.permute(0, 1, 4, 2, 5, 3).reshape(N, C, 8 * H, 8 * W)
 
+    def _decoder_mode(self, ctx: Tensor) -> str:
+        """How the refinement loop runs: "tf32" (fp32 CUDA net with TF32 matmuls AND convolutions allowed: every iteration on
+        our kernels, the tensor-core ones included), "strict" (fp32 CUDA net otherwise: token kernel + cuDNN fp32 convolutions
+        + the SepConvGRU glue kernels), "torch" (CPU golden runs, half-precision `native` runs: torch ops)."""
+        if not (self._native(ctx) and self.dec_dtype == torch.float32):
+            return "torch"
+        if torch.backends.cuda.matmul.allow_tf32 and torch.backends.cudnn.allow_tf32:
+            return "tf32"
+        return "strict"
+
     def memory_decoder(self, cost_memory: Tensor, context: Tensor, cost_maps: Tensor) -> tuple[Tensor, Tensor]:
         m, dd = "memory_decoder.", self.dec_dtype
         cost_memory = cost_memory.to(dd)
         B, _, H1, W1 = context.shape
-        N = H1 * W1
         coords0 = coords_grid(B, H1, W1, context.device, context.dtype)
         coords1, ccoords1 = coords0.clone(), coords0.clone()
         ctx = self._conv(context, m + "proj")
         net = ctx[:, :128].tanh().to(dd)
         cnet = net.clone()
         inp = ctx[:, 128:].relu().to(dd)
+        mode = self._decoder_mode(ctx)
         # GMA attention, once per frame (gma.py:39-82): softmax over the N x N similarity
         qk = self._conv(inp, m + "att.to_qk")
         qv = (qk[:, :128] * (128 ** -0.5)).flatten(2).transpose(1, 2)            # (B, N, 128)
         scores = torch.matmul(qv, qk[:, 128:].flatten(2))                        # (B, N, N)
-        fuse_att = (self._native(ctx) and dd == torch.float32 and torch.backends.cuda.matmul.allow_tf32
-                    and scores.shape[-1] % 4 == 0 and scores.shape[-1] <= 8192)
-        attention = None if fuse_att else scores.softmax(dim=-1)
+        # the N x N GMA attention matrix (184 MB at 640x480) is re-read by every iteration's aggregation GEMM, which is
+        # bound by that read: when TF32 matmuls are allowed it is kept in fp16 (values in [0, 1]; no precision below TF32's)
+        half_attention = mode != "torch" and torch.backends.cuda.matmul.allow_tf32
+        if half_attention and scores.shape[-1] % 4 == 0 and scores.shape[-1] <= 8192:
+            attention = self._ops.softmax_rows_f16(scores)         # softmax + fp16 in one pass over the scores
+        else:
+            attention = scores.softmax(dim=-1)
+            if half_attention:
+                attention = attention.to(torch.float16)
         ca = m + "decoder_layer.cross_attend."
         key = self._lin(cost_memory, ca + "k")
         value = self._lin(cost_memory, ca + "v")
-        ub, cu = m + "update_block.", m + "cov_update."
-        gamma = self.W[ub + "aggregator.gamma"]
-        P = B * N
-        native = self._native(ctx) and dd == torch.float32
-        # TF32 mode: both SepConvGRU units run on the tensor-core kernel (fp16 operands, fp32 state; csrc/gru_conv_tc.cu);
-        # strict mode keeps cuDNN's fp32 convolutions + the fused glue kernels
-        gru_tc = dec_tc = None
-        if native:
-            side = self._memo(("side_stream", ctx.device), lambda: torch.cuda.Stream(ctx.device))
-            as_map = lambda t: t.view(B, H1, W1, -1).permute(0, 3, 1, 2)                   # channels_last logical map
-            inp_rows = inp.permute(0, 2, 3, 1).reshape(P, 128).contiguous()
-            net_rows = net.permute(0, 2, 3, 1).reshape(P, 128).contiguous()
-        if native and torch.backends.cudnn.allow_tf32 and torch.backends.cuda.matmul.allow_tf32 and self.gru_tensor_cores:
-            def make_gru():
-                names = [f"conv{g}{o}" for g in ("zr", "q") for o in ("1", "2")]
-                ws = [{n: self.W[pre + "gru." + n + ".weight"] for n in names} for pre in (ub, cu)]
-                bs = [{n: self.W[pre + "gru." + n + ".bias"] for n in names} for pre in (ub, cu)]
-                return self._ops.SepConvGruTC(ws, bs, B, H1, W1, ctx.device)
-            gru_tc = self._memo(("gru_tc", B, H1, W1, ctx.device), make_gru)
-            dec_tc = self._memo(("decoder_tc", B, H1, W1, ctx.device), lambda: self._make_decoder_tc(B, H1, W1, ctx.device))
-            gru_tc.set_context(inp_rows)
-            gru_tc.set_state(0, net_rows)
-            gru_tc.set_state(1, net_rows)
-            net_d, cnet_d = gru_tc.h
-        elif native:
-            # recurrent state in NHWC [h | x] buffers (csrc/decoder_fused.cu): x = [inp | mf | mf + gamma*agg]
-            bufs = [torch.empty(P, 512, dtype=dd, device=ctx.device) for _ in range(4)]   # hx, rhx (flow) / hx, rhx (cov)
-            for bf in bufs:
-                bf[:, 128:256] = inp_rows
-            bufs[0][:, :128] = net_rows
-            bufs[2][:, :128] = bufs[0][:, :128]
-            zbuf, zbuf2 = torch.empty(P, 128, dtype=dd, device=ctx.device), torch.empty(P, 128, dtype=dd, device=ctx.device)
-            net_d, cnet_d = torch.empty(P, 128, dtype=dd, device=ctx.device), torch.empty(P, 128, dtype=dd, device=ctx.device)
-        # the N x N GMA attention matrix (184 MB at 640x480) is re-read by every iteration's aggregation GEMM, which is
-        # bound by that read: when TF32 matmuls are allowed it is kept in fp16 (values in [0, 1]; no precision below TF32's)
-        if fuse_att:
-            attention_h = self._ops.softmax_rows_f16(scores)       # softmax + fp16 in one pass over the scores
-        else:
-            attention_h = attention.to(torch.float16) if native and torch.backends.cuda.matmul.allow_tf32 else None
-        fast_tokens = native and QUERY_DIM == 64 and self.lookup_fn is self._ops.corr_lookup
-        if fast_tokens:
-            token_blob = self._memo(("token_blob", ctx.device), lambda: self._ops.decoder_token_blob(self.W, m))
-            key, value = key.contiguous(), value.contiguous()
-        use_tc = dec_tc is not None and fast_tokens and attention_h is not None and self.conv_tensor_cores
-        cov_done = None
-        if use_tc:
-            side2 = self._memo(("side_stream2", ctx.device), lambda: torch.cuda.Stream(ctx.device))
-        for _ in range(self.depth):
-            if use_tc:
-                # TF32 mode: the whole iteration on our kernels — lookup, token kernel, motion encoder / value projection / heads
-                # on the tensor-core convolution kernel (fp16 rows between the layers), SepConvGRU on its tensor-core kernel; the one
-                # library call left is the GMA aggregation GEMM
-                ops, t, shp = self._ops, dec_tc, (B, H1, W1)
-                main = torch.cuda.current_stream()
-                fork = torch.cuda.Event()
-                fork.record(main)
-                with torch.cuda.stream(side):                                                # flow branch of the motion encoder
-                    side.wait_event(fork)
-                    ops.flow_im2col(coords1, coords0, t.f0, t.mf32, t.mf16)
-                    ops.conv_tc(t.f0, t.convf1[0], t.convf1[1], 128, 1, True, shp, in_dense=True, out16=t.f1)
-                    ops.conv_tc(t.f1, t.convf2[0], t.convf2[1], 64, 3, True, shp, out16=t.cp, out16_offset=192)
-                    joinf = torch.cuda.Event()
-                    joinf.record(side)
-                cf = ops.corr_lookup(cost_maps, coords1, rows=True)                          # (P, 81)
-                ops.decoder_token(cf, coords1, key, value, token_blob, out16_rows=t.tok16)   # rows [global | forward | 0] in fp16
-                ops.conv_tc(t.tok16, t.convc1[0], t.convc1[1], 256, 1, True, shp, out16=t.c1)
-                ops.conv_tc(t.c1, t.convc2[0], t.convc2[1], 192, 3, True, shp, out16=t.cp)
-                main.wait_event(joinf)
-                ops.conv_tc(t.cp, t.conv[0], t.conv[1], 126, 3, True, shp, out16=t.mf16, out32=t.mf32)   # + flow in channels 126, 127
-                ops.conv_tc(t.mf16, t.to_v[0], None, 128, 1, False, shp, out16=t.v16, out16_dense=True)
-                agg = torch.bmm(attention_h, t.v16.view(B, N, 128), out_dtype=torch.float32)  # GMA aggregation (gma.py:84-130)
-                if cov_done is not None:            # the previous iteration's covariance head still reads the covariance unit's state rows
-                    main.wait_event(cov_done)
-                # one launch chain per GRU unit on two streams (a joint launch is 168 CTAs = two waves per stage); the covariance
-                # unit's chain ends in `unit1_done`, which only the covariance head waits for
-                unit1_done = gru_tc.step(t.mf32, agg.view(P, 128), gamma, split_units=self.gru_split_units, join=False)
-                if unit1_done is None:
-                    unit1_done = torch.cuda.Event()
-                    unit1_done.record(main)
-                # The covariance head (4 chained convolutions, covhead.py:20-58) feeds only the covariance coordinates: it runs on
-                # its own stream and is joined right before the NEXT iteration's GRU update, so it overlaps the next lookup / token
-                # kernel / motion encoder instead of extending this iteration (they depend on the flow head only).
-                with torch.cuda.stream(side2):
-                    side2.wait_event(unit1_done)
-                    ops.conv_tc(gru_tc.h_rows[0][1], t.chw[0][0], t.chw[0][1], 256, 3, True, shp, out16=t.ch1)
-                    ops.conv_tc(t.ch1, t.chw[1][0], t.chw[1][1], 128, 3, False, shp, out16=t.ch2)
-                    ops.conv_tc(t.ch2, t.chw[2][0], t.chw[2][1], 64, 3, True, shp, out16=t.ch3)
-                    ops.conv_tc(t.ch3, t.chw[3][0], t.chw[3][1], 2, 3, False, shp, add_to_map=ccoords1)   # ccoords1 += delta (in the epilogue)
-                    cov_done = torch.cuda.Event()
-                    cov_done.record(side2)
-                ops.conv_tc(gru_tc.h_rows[0][0], t.fh1[0], t.fh1[1], 256, 3, True, shp, out16=t.fh)
-                ops.conv_tc(t.fh, t.fh2[0], t.fh2[1], 2, 3, False, shp, add_to_map=coords1)               # coords1 += delta_flow
-                if self.taps is not None:
-                    main.wait_event(cov_done)
-                net, cnet = as_map(net_d), as_map(cnet_d)
-                self._tap("flow_iter", coords1 - coords0)
-                self._tap("cov_iter", ccoords1 - coords0)
-                continue
-            flow = (coords1 - coords0).to(dd)
-            if native and fast_tokens:
-                # pixels-major rows end to end: lookup kernel -> ONE token kernel (token MLP, LayerNorm + sine embedding, q
-                # projection, per-pixel 8x8 cross attention, output projection, FFN) writing the motion encoder's input rows
-                cf = self._ops.corr_lookup(cost_maps, coords1, rows=True)                     # (P, 81)
-                corr = self._ops.decoder_token(cf, coords1, key, value, token_blob)           # (P, 160) = [global | forward | 0]
-                corr = corr.view(B, H1, W1, 160).permute(0, 3, 1, 2)                          # channels_last view
-                convc1 = "convc1p"
-            else:
-                cost_forward = self.lookup_fn(cost_maps, coords1).to(dd)         # fp32 lookup (covhead.py:91-93)
-                query = self._conv(F.gelu(self._conv(cost_forward, m + "flow_token_encoder.0")), m + "flow_token_encoder.2")
-                query = query.permute(0, 2, 3, 1).reshape(P, QUERY_DIM)          # rows = pixels (2-D: plain GEMMs below)
-                # cross attention of each pixel's query to its 8 cost-memory tokens (decoder.py:56-76)
-                enc = sine_embed(coords1.to(dd).permute(0, 2, 3, 1).reshape(P, 2), QUERY_DIM)
-                qin = self._ln(query, ca + "norm1") + enc
-                q = self._lin(qin, ca + "q")
-                a = self._attn(q.unsqueeze(1), key, value, 8).squeeze(1)
-                g = query + self._lin(torch.cat([a, query], dim=1), ca + "proj")
-                g = g + self._lin(F.gelu(self._lin(self._ln(g, ca + "norm2"), ca + "ffn.0")), ca + "ffn.3")
-                cost_global = g.view(B, H1, W1, QUERY_DIM).permute(0, 3, 1, 2)
-                corr = torch.cat([cost_global, cost_forward], dim=1)
-                convc1 = "convc1"
-            # motion encoder (gru.py:45-64)
-            e = ub + "encoder."
-            if native:                                               # flow branch of the motion encoder on the side stream
-                main = torch.cuda.current_stream()
-                fork = torch.cuda.Event()
-                fork.record(main)
-                with torch.cuda.stream(side):
-                    side.wait_event(fork)
-                    flo = self._conv_relu(self._conv_relu(flow, e + "convf1", padding=3), e + "convf2", padding=1)
-                    joinf = torch.cuda.Event()
-                    joinf.record(side)
-                cor = self._conv_relu(self._conv_relu(corr, e + convc1), e + "convc2", padding=1)
-                main.wait_event(joinf)
-            else:
-                cor = self._conv_relu(self._conv_relu(corr, e + convc1), e + "convc2", padding=1)
-                flo = self._conv_relu(self._conv_relu(flow, e + "convf1", padding=3), e + "convf2", padding=1)
-            if native:      # 128-channel conv output (last two channels zero), flow written into them in place
-                mf = self._conv_relu(torch.cat([cor, flo], dim=1), e + "convp", padding=1)
-                mf.permute(0, 2, 3, 1)[..., 126:] = flow.permute(0, 2, 3, 1)
-            else:
-                mf = torch.cat([self._conv_relu(torch.cat([cor, flo], dim=1), e + "conv", padding=1), flow], dim=1)
-            # GMA aggregation (gma.py:84-130)
-            mf = mf.contiguous(memory_format=torch.channels_last)
-            v = self._conv(mf, ub + "aggregator.to_v").flatten(2).transpose(1, 2)   # (B, N, 128)
-            if attention_h is not None:     # fp16 operands (11-bit mantissa >= TF32's 10), fp32 accumulate AND fp32 output
-                agg = torch.bmm(attention_h, v.to(torch.float16), out_dtype=torch.float32)
-            else:
-                agg = torch.matmul(attention, v)                                    # (B, N, 128) = pixels-major
-            if native:
-                # the flow branch (GRU + flow head) and the covariance branch (GRU + cov head) only share their input:
-                # at 60x80 each conv fills about two thirds of the 132 SMs, so the two run on forked streams (fork/join is
-                # captured into the CUDA graph as parallel branches)
-                if gru_tc is not None:
-                    gru_tc.step(mf.permute(0, 2, 3, 1), agg, gamma)              # both units, 5 launches
-                else:
-                    self._ops.gru_input(mf.permute(0, 2, 3, 1), agg, gamma, bufs)
-                main = torch.cuda.current_stream()
-                fork = torch.cuda.Event()
-                fork.record(main)
-                with torch.cuda.stream(side):
-                    side.wait_event(fork)
-                    if gru_tc is None:
-                        self._gru_native(bufs[2], bufs[3], zbuf2, cu + "gru.", cnet_d, (B, H1, W1))
-                    cnet = as_map(cnet_d)
-                    h = cu + "cov_head."
-                    t = self._conv(self._conv_relu(cnet, h + "conv1", padding=1), h + "conv2", padding=1)
-                    d_cov = self._conv(self._conv_relu(t, h + "conv3", padding=1), h + "conv4", padding=1)
-                    join = torch.cuda.Event()
-                    join.record(side)
-                if gru_tc is None:
-                    self._gru_native(bufs[0], bufs[1], zbuf, ub + "gru.", net_d, (B, H1, W1))
-                net = as_map(net_d)
-                d_flow = self._conv(self._conv_relu(net, ub + "flow_head.conv1", padding=1), ub + "flow_head.conv2", padding=1)
-                main.wait_event(join)
-            else:
-                inp_cat = torch.cat([inp, mf, mf + gamma * agg.transpose(1, 2).reshape(B, 128, H1, W1)], dim=1)
-                net = self._gru(net, inp_cat, ub + "gru.")
-                cnet = self._gru(cnet, inp_cat, cu + "gru.")
-                d_flow = self._conv(self._conv_relu(net, ub + "flow_head.conv1", padding=1), ub + "flow_head.conv2", padding=1)
-                h = cu + "cov_head."
-                t = self._conv(self._conv_relu(cnet, h + "conv1", padding=1), h + "conv2", padding=1)
-                d_cov = self._conv(self._conv_relu(t, h + "conv3", padding=1), h + "conv4", padding=1)
-            coords1 = coords1 + _f32(d_flow)
-            ccoords1 = ccoords1 + _f32(d_cov)
-            self._tap("flow_iter", coords1 - coords0)
-            self._tap("cov_iter", ccoords1 - coords0)
-        if cov_done is not None:
-            torch.cuda.current_stream().wait_event(cov_done)
+        refine = {"tf32": self._refine_tf32, "strict": self._refine_strict, "torch": self._refine_torch}[mode]
+        coords1, ccoords1, net, cnet = refine(coords0, coords1, ccoords1, net, cnet, inp, attention, key, value, cost_maps)
         # the reference evaluates both mask heads + upsampling every iteration but (eval mode) returns
         # only the last one (covhead.py:137-140) -> evaluate once
-        if native:      # scale + softmax + unfold + weighted sum + pixel shuffle in one kernel per map
+        ub, cu = m + "update_block.", m + "cov_update."
+        if mode != "torch":     # scale + softmax + unfold + weighted sum + pixel shuffle in one kernel per map
             up_logits = self._conv(self._conv_relu(net, ub + "mask.0", padding=1), ub + "mask.2")
             cov_logits = self._conv(self._conv_relu(cnet, cu + "mask.0", padding=1), cu + "mask.2")
             return (self._ops.convex_upsample(coords1 - coords0, up_logits, 0.25),
@@ -928,6 +757,205 @@ class FlowFormerCovNet:
         up_mask = _f32(0.25 * self._conv(F.relu(self._conv(net, ub + "mask.0", padding=1)), ub + "mask.2"))
         cov_mask = _f32(0.25 * self._conv(F.relu(self._conv(cnet, cu + "mask.0", padding=1)), cu + "mask.2"))
         return self.convex_upsample(coords1 - coords0, up_mask), self.convex_upsample(ccoords1 - coords0, cov_mask)
+
+    def _refine_tf32(self, coords0, coords1, ccoords1, net, cnet, inp, attention, key, value, cost_maps):
+        """The whole iteration on our kernels: lookup, token kernel, motion encoder / value projection / heads on the
+        tensor-core convolution kernel (fp16 rows between the layers), both SepConvGRU units on their tensor-core kernel (fp16
+        operands, fp32 state; csrc/gru_conv_tc.cu); the one library call left is the GMA aggregation GEMM over the fp16
+        `attention`."""
+        m = "memory_decoder."
+        ub, cu = m + "update_block.", m + "cov_update."
+        ops = self._ops
+        B, _, H1, W1 = coords0.shape
+        N, dev = H1 * W1, coords0.device
+        P, shp = B * N, (B, H1, W1)
+        side = self._memo(("side_stream", dev), lambda: torch.cuda.Stream(dev))
+        side2 = self._memo(("side_stream2", dev), lambda: torch.cuda.Stream(dev))
+        as_map = lambda t: t.view(B, H1, W1, -1).permute(0, 3, 1, 2)                   # channels_last logical map
+
+        def make_gru():
+            names = [f"conv{g}{o}" for g in ("zr", "q") for o in ("1", "2")]
+            ws = [{n: self.W[pre + "gru." + n + ".weight"] for n in names} for pre in (ub, cu)]
+            bs = [{n: self.W[pre + "gru." + n + ".bias"] for n in names} for pre in (ub, cu)]
+            return ops.SepConvGruTC(ws, bs, B, H1, W1, dev)
+        gru = self._memo(("gru_tc", B, H1, W1, dev), make_gru)
+        t = self._memo(("decoder_tc", B, H1, W1, dev), lambda: self._make_decoder_tc(B, H1, W1, dev))
+        gru.set_context(inp.permute(0, 2, 3, 1).reshape(P, 128).contiguous())
+        net_rows = net.permute(0, 2, 3, 1).reshape(P, 128).contiguous()
+        gru.set_state(0, net_rows)
+        gru.set_state(1, net_rows)
+        net_d, cnet_d = gru.h
+        token_blob = self._memo(("token_blob", dev), lambda: ops.decoder_token_blob(self.W, m))
+        key, value = key.contiguous(), value.contiguous()
+        gamma = self.W[ub + "aggregator.gamma"]
+        cov_done = None
+        for _ in range(self.depth):
+            main = torch.cuda.current_stream()
+            fork = torch.cuda.Event()
+            fork.record(main)
+            with torch.cuda.stream(side):                                                # flow branch of the motion encoder
+                side.wait_event(fork)
+                ops.flow_im2col(coords1, coords0, t.f0, t.mf32, t.mf16)
+                ops.conv_tc(t.f0, t.convf1[0], t.convf1[1], 128, 1, True, shp, in_dense=True, out16=t.f1)
+                ops.conv_tc(t.f1, t.convf2[0], t.convf2[1], 64, 3, True, shp, out16=t.cp, out16_offset=192)
+                joinf = torch.cuda.Event()
+                joinf.record(side)
+            cf = ops.corr_lookup(cost_maps, coords1, rows=True)                          # (P, 81)
+            ops.decoder_token(cf, coords1, key, value, token_blob, out16_rows=t.tok16)   # rows [global | forward | 0] in fp16
+            ops.conv_tc(t.tok16, t.convc1[0], t.convc1[1], 256, 1, True, shp, out16=t.c1)
+            ops.conv_tc(t.c1, t.convc2[0], t.convc2[1], 192, 3, True, shp, out16=t.cp)
+            main.wait_event(joinf)
+            ops.conv_tc(t.cp, t.conv[0], t.conv[1], 126, 3, True, shp, out16=t.mf16, out32=t.mf32)   # + flow in channels 126, 127
+            ops.conv_tc(t.mf16, t.to_v[0], None, 128, 1, False, shp, out16=t.v16, out16_dense=True)
+            agg = torch.bmm(attention, t.v16.view(B, N, 128), out_dtype=torch.float32)   # GMA aggregation (gma.py:84-130)
+            if cov_done is not None:            # the previous iteration's covariance head still reads the covariance unit's state rows
+                main.wait_event(cov_done)
+            # one launch chain per GRU unit on two streams; the covariance unit's chain ends in `unit1_done`, which only the
+            # covariance head waits for
+            unit1_done = gru.step(t.mf32, agg.view(P, 128), gamma)
+            # The covariance head (4 chained convolutions, covhead.py:20-58) feeds only the covariance coordinates: it runs on
+            # its own stream and is joined right before the NEXT iteration's GRU update, so it overlaps the next lookup / token
+            # kernel / motion encoder instead of extending this iteration (they depend on the flow head only).
+            with torch.cuda.stream(side2):
+                side2.wait_event(unit1_done)
+                ops.conv_tc(gru.h_rows[0][1], t.chw[0][0], t.chw[0][1], 256, 3, True, shp, out16=t.ch1)
+                ops.conv_tc(t.ch1, t.chw[1][0], t.chw[1][1], 128, 3, False, shp, out16=t.ch2)
+                ops.conv_tc(t.ch2, t.chw[2][0], t.chw[2][1], 64, 3, True, shp, out16=t.ch3)
+                ops.conv_tc(t.ch3, t.chw[3][0], t.chw[3][1], 2, 3, False, shp, add_to_map=ccoords1)   # ccoords1 += delta (in the epilogue)
+                cov_done = torch.cuda.Event()
+                cov_done.record(side2)
+            ops.conv_tc(gru.h_rows[0][0], t.fh1[0], t.fh1[1], 256, 3, True, shp, out16=t.fh)
+            ops.conv_tc(t.fh, t.fh2[0], t.fh2[1], 2, 3, False, shp, add_to_map=coords1)               # coords1 += delta_flow
+            if self.taps is not None:
+                main.wait_event(cov_done)
+            net, cnet = as_map(net_d), as_map(cnet_d)
+            self._tap("flow_iter", coords1 - coords0)
+            self._tap("cov_iter", ccoords1 - coords0)
+        if cov_done is not None:
+            torch.cuda.current_stream().wait_event(cov_done)
+        return coords1, ccoords1, net, cnet
+
+    def _refine_strict(self, coords0, coords1, ccoords1, net, cnet, inp, attention, key, value, cost_maps):
+        """fp32 everywhere the flags ask for it: lookup and token kernel rows into cuDNN's convolutions, SepConvGRU as cuDNN
+        convolutions + the glue kernels of csrc/decoder_fused.cu on NHWC `[h | x]` state buffers. `attention` is fp16 when
+        TF32 matmuls are allowed (the aggregation then reads it like the tf32 mode does), fp32 otherwise."""
+        m, dd = "memory_decoder.", torch.float32
+        ub, cu, e = m + "update_block.", m + "cov_update.", m + "update_block.encoder."
+        ops = self._ops
+        B, _, H1, W1 = coords0.shape
+        P, dev = B * H1 * W1, coords0.device
+        side = self._memo(("side_stream", dev), lambda: torch.cuda.Stream(dev))
+        as_map = lambda t: t.view(B, H1, W1, -1).permute(0, 3, 1, 2)                   # channels_last logical map
+        inp_rows = inp.permute(0, 2, 3, 1).reshape(P, 128).contiguous()
+        net_rows = net.permute(0, 2, 3, 1).reshape(P, 128).contiguous()
+        # recurrent state in NHWC [h | x] buffers (csrc/decoder_fused.cu): x = [inp | mf | mf + gamma*agg]
+        bufs = [torch.empty(P, 512, dtype=dd, device=dev) for _ in range(4)]   # hx, rhx (flow) / hx, rhx (cov)
+        for bf in bufs:
+            bf[:, 128:256] = inp_rows
+        bufs[0][:, :128] = net_rows
+        bufs[2][:, :128] = bufs[0][:, :128]
+        zbuf, zbuf2 = torch.empty(P, 128, dtype=dd, device=dev), torch.empty(P, 128, dtype=dd, device=dev)
+        net_d, cnet_d = torch.empty(P, 128, dtype=dd, device=dev), torch.empty(P, 128, dtype=dd, device=dev)
+        token_blob = self._memo(("token_blob", dev), lambda: ops.decoder_token_blob(self.W, m))
+        key, value = key.contiguous(), value.contiguous()
+        gamma = self.W[ub + "aggregator.gamma"]
+        for _ in range(self.depth):
+            flow = coords1 - coords0
+            # pixels-major rows end to end: lookup kernel -> ONE token kernel (token MLP, LayerNorm + sine embedding, q
+            # projection, per-pixel 8x8 cross attention, output projection, FFN) writing the motion encoder's input rows
+            cf = ops.corr_lookup(cost_maps, coords1, rows=True)                          # (P, 81)
+            corr = ops.decoder_token(cf, coords1, key, value, token_blob)                # (P, 160) = [global | forward | 0]
+            corr = corr.view(B, H1, W1, 160).permute(0, 3, 1, 2)                         # channels_last view
+            # motion encoder (gru.py:45-64), its flow branch on the side stream
+            main = torch.cuda.current_stream()
+            fork = torch.cuda.Event()
+            fork.record(main)
+            with torch.cuda.stream(side):
+                side.wait_event(fork)
+                flo = self._conv_relu(self._conv_relu(flow, e + "convf1", padding=3), e + "convf2", padding=1)
+                joinf = torch.cuda.Event()
+                joinf.record(side)
+            cor = self._conv_relu(self._conv_relu(corr, e + "convc1p"), e + "convc2", padding=1)
+            main.wait_event(joinf)
+            # 128-channel conv output (last two channels zero), flow written into them in place
+            mf = self._conv_relu(torch.cat([cor, flo], dim=1), e + "convp", padding=1)
+            mf.permute(0, 2, 3, 1)[..., 126:] = flow.permute(0, 2, 3, 1)
+            # GMA aggregation (gma.py:84-130)
+            mf = mf.contiguous(memory_format=torch.channels_last)
+            v = self._conv(mf, ub + "aggregator.to_v").flatten(2).transpose(1, 2)   # (B, N, 128)
+            if attention.dtype == torch.float16:      # fp16 operands (11-bit mantissa >= TF32's 10), fp32 accumulate AND output
+                agg = torch.bmm(attention, v.to(torch.float16), out_dtype=torch.float32)
+            else:
+                agg = torch.matmul(attention, v)                                    # (B, N, 128) = pixels-major
+            # the flow branch (GRU + flow head) and the covariance branch (GRU + cov head) only share their input:
+            # at 60x80 each conv fills about two thirds of the 132 SMs, so the two run on forked streams (fork/join is
+            # captured into the CUDA graph as parallel branches)
+            ops.gru_input(mf.permute(0, 2, 3, 1), agg, gamma, bufs)
+            main = torch.cuda.current_stream()
+            fork = torch.cuda.Event()
+            fork.record(main)
+            with torch.cuda.stream(side):
+                side.wait_event(fork)
+                self._gru_native(bufs[2], bufs[3], zbuf2, cu + "gru.", cnet_d, (B, H1, W1))
+                cnet = as_map(cnet_d)
+                h = cu + "cov_head."
+                t = self._conv(self._conv_relu(cnet, h + "conv1", padding=1), h + "conv2", padding=1)
+                d_cov = self._conv(self._conv_relu(t, h + "conv3", padding=1), h + "conv4", padding=1)
+                join = torch.cuda.Event()
+                join.record(side)
+            self._gru_native(bufs[0], bufs[1], zbuf, ub + "gru.", net_d, (B, H1, W1))
+            net = as_map(net_d)
+            d_flow = self._conv(self._conv_relu(net, ub + "flow_head.conv1", padding=1), ub + "flow_head.conv2", padding=1)
+            main.wait_event(join)
+            coords1 = coords1 + d_flow
+            ccoords1 = ccoords1 + d_cov
+            self._tap("flow_iter", coords1 - coords0)
+            self._tap("cov_iter", ccoords1 - coords0)
+        return coords1, ccoords1, net, cnet
+
+    def _refine_torch(self, coords0, coords1, ccoords1, net, cnet, inp, attention, key, value, cost_maps):
+        """torch ops in the decoder dtype, `lookup_fn` for the window lookup: the CPU golden runs (float32 / float64) and the
+        half-precision `native` runs."""
+        m, dd = "memory_decoder.", self.dec_dtype
+        ub, cu, e = m + "update_block.", m + "cov_update.", m + "update_block.encoder."
+        ca = m + "decoder_layer.cross_attend."
+        B, _, H1, W1 = coords0.shape
+        P = B * H1 * W1
+        gamma = self.W[ub + "aggregator.gamma"]
+        for _ in range(self.depth):
+            flow = (coords1 - coords0).to(dd)
+            cost_forward = self.lookup_fn(cost_maps, coords1).to(dd)         # fp32 lookup (covhead.py:91-93)
+            query = self._conv(F.gelu(self._conv(cost_forward, m + "flow_token_encoder.0")), m + "flow_token_encoder.2")
+            query = query.permute(0, 2, 3, 1).reshape(P, QUERY_DIM)          # rows = pixels (2-D: plain GEMMs below)
+            # cross attention of each pixel's query to its 8 cost-memory tokens (decoder.py:56-76)
+            enc = sine_embed(coords1.to(dd).permute(0, 2, 3, 1).reshape(P, 2), QUERY_DIM)
+            qin = self._ln(query, ca + "norm1") + enc
+            q = self._lin(qin, ca + "q")
+            a = self._attn(q.unsqueeze(1), key, value, 8).squeeze(1)
+            g = query + self._lin(torch.cat([a, query], dim=1), ca + "proj")
+            g = g + self._lin(F.gelu(self._lin(self._ln(g, ca + "norm2"), ca + "ffn.0")), ca + "ffn.3")
+            cost_global = g.view(B, H1, W1, QUERY_DIM).permute(0, 3, 1, 2)
+            corr = torch.cat([cost_global, cost_forward], dim=1)
+            # motion encoder (gru.py:45-64)
+            cor = self._conv_relu(self._conv_relu(corr, e + "convc1"), e + "convc2", padding=1)
+            flo = self._conv_relu(self._conv_relu(flow, e + "convf1", padding=3), e + "convf2", padding=1)
+            mf = torch.cat([self._conv_relu(torch.cat([cor, flo], dim=1), e + "conv", padding=1), flow], dim=1)
+            # GMA aggregation (gma.py:84-130)
+            mf = mf.contiguous(memory_format=torch.channels_last)
+            v = self._conv(mf, ub + "aggregator.to_v").flatten(2).transpose(1, 2)   # (B, N, 128)
+            agg = torch.matmul(attention, v)                                    # (B, N, 128) = pixels-major
+            inp_cat = torch.cat([inp, mf, mf + gamma * agg.transpose(1, 2).reshape(B, 128, H1, W1)], dim=1)
+            net = self._gru(net, inp_cat, ub + "gru.")
+            cnet = self._gru(cnet, inp_cat, cu + "gru.")
+            d_flow = self._conv(self._conv_relu(net, ub + "flow_head.conv1", padding=1), ub + "flow_head.conv2", padding=1)
+            h = cu + "cov_head."
+            t = self._conv(self._conv_relu(cnet, h + "conv1", padding=1), h + "conv2", padding=1)
+            d_cov = self._conv(self._conv_relu(t, h + "conv3", padding=1), h + "conv4", padding=1)
+            coords1 = coords1 + _f32(d_flow)
+            ccoords1 = ccoords1 + _f32(d_cov)
+            self._tap("flow_iter", coords1 - coords0)
+            self._tap("cov_iter", ccoords1 - coords0)
+        return coords1, ccoords1, net, cnet
 
     # ---- top level (flownet.py:18-44) -----------------------------------------------------------
     @torch.inference_mode()

@@ -91,7 +91,6 @@ EXPORTS = {
     "macvo_patch_embed_conv1": (C.c_int, [C.c_void_p] * 4 + [C.c_longlong, C.c_int, C.c_int, C.c_int, C.c_void_p]),
     "macvo_add_rows_relu": (C.c_int, [C.c_void_p] * 2 + [C.c_longlong, C.c_int, C.c_int, C.c_void_p]),
     "macvo_small_attention": (C.c_int, [C.c_void_p] * 4 + [C.c_int] * 7 + [C.c_void_p]),
-    "macvo_query_prep": (C.c_int, [C.c_void_p] * 6 + [C.c_int, C.c_int, C.c_float, C.c_void_p]),
     "macvo_small_attention_ex": (C.c_int, [C.c_void_p] * 4 + [C.c_int] * 10 + [C.c_void_p] * 2 + [C.c_int, C.c_void_p]),
     "macvo_latent_pool": (C.c_int, [C.c_void_p] * 5 + [C.c_longlong, C.c_int, C.c_void_p]),
     "macvo_decoder_token_blob_floats": (C.c_size_t, []),
@@ -103,14 +102,11 @@ EXPORTS = {
     "macvo_softmax_rows_f16": (C.c_int, [C.c_void_p] * 2 + [C.c_longlong, C.c_int, C.c_void_p]),
     "macvo_convex_upsample": (C.c_int, [C.c_void_p] * 3 + [C.c_float] + [C.c_int] * 3 + [C.c_void_p]),
     "macvo_rows_count": (C.c_size_t, [C.c_int] * 4),
-    "macvo_tc_set_timeline": (None, [C.c_void_p, C.c_int]),
-    "macvo_conv_tc_set_trace": (None, [C.c_void_p]),
     "macvo_conv_tc": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p] + [C.c_int] * 7
                       + [C.c_void_p] + [C.c_int] * 3 + [C.c_void_p] + [C.c_int] * 3 + [C.c_void_p]),
     "macvo_flow_im2col": (C.c_int, [C.c_void_p] * 5 + [C.c_int] * 3 + [C.c_void_p]),
     "macvo_gru_tc_operand_rows": (C.c_size_t, [C.c_int] * 4),
-    "macvo_gru_tc_set_trace": (None, [C.c_void_p]),
-    "macvo_gru_tc_stage": (C.c_int, [C.c_int] * 6 + [C.c_void_p] * 8),
+    "macvo_gru_tc_stage": (C.c_int, [C.c_int] * 5 + [C.c_void_p] * 8),
     "macvo_gru_tc_pack": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p] + [C.c_int] * 6 + [C.c_void_p]),
     "macvo_gru_tc_pack_motion": (C.c_int, [C.c_void_p] * 5 + [C.c_int] * 3 + [C.c_void_p]),
     "macvo_posenet_input": (C.c_int, [C.c_void_p] * 2 + [C.c_int] * 2 + [C.c_double, C.c_void_p, C.c_void_p]),
@@ -1001,28 +997,30 @@ def pack_rows(src: Tensor, dst: Tensor, offset: int, shape: tuple[int, int, int]
 
 
 class SepConvGruTC:
-    """The decoder's SepConvGRU units (gru.py:22-43; flow + covariance, covhead.py:95-131) on the tensor-core path
+    """The decoder's two SepConvGRU units (gru.py:22-43; flow + covariance, covhead.py:95-131) on the tensor-core path
     (csrc/gru_conv_tc.cu): fp32 recurrent state `h[u]` (pixels, 128) in dense pixel order, fp16 padded operand rows for the two
-    passes, one `step` = pack the motion features + 4 kernel launches for all units.
+    passes, one `step` = pack the motion features + one 4-launch chain per unit.
 
     weights[u]: {"convzr1": (256,512,1,5), "convq1": (128,512,1,5), "convzr2": (256,512,5,1), "convq2": (128,512,5,1)} fp32
-    filters with the z | r filters concatenated, biases[u]: the matching (N,) vectors."""
+    filters with the z | r filters concatenated, biases[u]: the matching (N,) vectors; u = 0 flow, 1 covariance."""
+
+    UNITS = 2
 
     def __init__(self, weights: list[dict], biases: list[dict], batch: int, height: int, width: int, device):
         lib = load_library()
-        self.units, self.shape, self.device = len(weights), (int(batch), int(height), int(width)), device
-        if self.units not in (1, 2):
-            raise MacvoB200Error("SepConvGruTC: 1 or 2 units")
+        self.shape, self.device = (int(batch), int(height), int(width)), device
+        if len(weights) != self.UNITS or len(biases) != self.UNITS:
+            raise MacvoB200Error("SepConvGruTC: expects the decoder's two units (flow, covariance)")
         P = batch * height * width
         rows = [int(lib.macvo_gru_tc_operand_rows(batch, height, width, o)) for o in (0, 1)]
         f16 = dict(dtype=torch.float16, device=device)
         self.x = [torch.zeros(r, 3 * GRU_HID, **f16) for r in rows]
-        self.h_rows = [[torch.zeros(r, GRU_HID, **f16) for _ in range(self.units)] for r in rows]     # [pass][unit]
-        self.rh_rows = [[torch.zeros(r, GRU_HID, **f16) for _ in range(self.units)] for r in rows]
-        self.h = [torch.zeros(P, GRU_HID, dtype=torch.float32, device=device) for _ in range(self.units)]
-        self.z = [torch.zeros(P, GRU_HID, dtype=torch.float32, device=device) for _ in range(self.units)]
+        self.h_rows = [[torch.zeros(r, GRU_HID, **f16) for _ in range(self.UNITS)] for r in rows]     # [pass][unit]
+        self.rh_rows = [[torch.zeros(r, GRU_HID, **f16) for _ in range(self.UNITS)] for r in rows]
+        self.h = [torch.zeros(P, GRU_HID, dtype=torch.float32, device=device) for _ in range(self.UNITS)]
+        self.z = [torch.zeros(P, GRU_HID, dtype=torch.float32, device=device) for _ in range(self.UNITS)]
         self.w, self.b = {}, {}
-        for u in range(self.units):
+        for u in range(self.UNITS):
             for o in (0, 1):
                 for st, name in ((0, f"convzr{o + 1}"), (1, f"convq{o + 1}")):
                     w = weights[u][name].detach().to(device=device, dtype=torch.float32)
@@ -1031,17 +1029,12 @@ class SepConvGruTC:
                         raise MacvoB200Error(f"SepConvGruTC: unexpected filter shape {tuple(w.shape)} for {name}")
                     self.w[u, o, st] = w.reshape(n, GRU_IN, 5).permute(0, 2, 1).reshape(n, 5 * GRU_IN).to(torch.float16).contiguous()
                     self.b[u, o, st] = biases[u][name].detach().to(device=device, dtype=torch.float32).contiguous()
-        ptrs = lambda ts: (C.c_void_p * 2)(*[t.data_ptr() for t in ts], *([None] * (2 - len(ts))))
-        self._args = {(o, st): (ptrs(self.h_rows[o] if st == 0 else self.rh_rows[o]), self.x[o].data_ptr(),
-                                ptrs([self.w[u, o, st] for u in range(self.units)]), ptrs([self.b[u, o, st] for u in range(self.units)]),
-                                ptrs(self.h), ptrs(self.z), ptrs(self.rh_rows[o] if st == 0 else self.h_rows[1 - o]))
-                      for o in (0, 1) for st in (0, 1)}
-        one = lambda t: (C.c_void_p * 2)(t.data_ptr(), None)
-        self._unit_args = {(u, o, st): (one((self.h_rows[o] if st == 0 else self.rh_rows[o])[u]), self.x[o].data_ptr(),
-                                        one(self.w[u, o, st]), one(self.b[u, o, st]), one(self.h[u]), one(self.z[u]),
-                                        one((self.rh_rows[o] if st == 0 else self.h_rows[1 - o])[u]))
-                           for u in range(self.units) for o in (0, 1) for st in (0, 1)}
-        self._side = torch.cuda.Stream(device) if self.units == 2 else None
+        # device pointers of every (unit, pass, stage) launch: h | r*h rows in, x rows, filters, bias, state, z, rows out
+        self._stage_args = {(u, o, st): ((self.h_rows[o] if st == 0 else self.rh_rows[o])[u].data_ptr(), self.x[o].data_ptr(),
+                                         self.w[u, o, st].data_ptr(), self.b[u, o, st].data_ptr(), self.h[u].data_ptr(),
+                                         self.z[u].data_ptr(), (self.rh_rows[o] if st == 0 else self.h_rows[1 - o])[u].data_ptr())
+                            for u in range(self.UNITS) for o in (0, 1) for st in (0, 1)}
+        self._side = torch.cuda.Stream(device)
 
     def _pack(self, src: Tensor, dst: Tensor, offset: int, vertical: int) -> None:
         B, H, W = self.shape
@@ -1061,48 +1054,39 @@ class SepConvGruTC:
         self.h[unit].copy_(_dense(h_rows, GRU_HID, "SepConvGruTC state").view(-1, GRU_HID))
         self._pack(self.h[unit], self.h_rows[0][unit], 0, 0)
 
-    def step(self, mf: Tensor, agg: Tensor, gamma: Tensor, split_units: bool = False, join: bool = True):
-        """one SepConvGRU update of every unit with x = [inp | mf | mf + gamma * agg]; new state in `self.h[u]`.
-        split_units: one 4-launch chain per unit on two streams instead of 4 launches covering both units — with 84 CTA tiles per
-        unit (640x480: two 60x80 maps) a joint launch is 168 CTAs = two waves on 132 SMs per stage, two independent chains of
-        84-CTA launches keep the SMs filled across the stage boundaries. With join=False the current stream only carries
-        unit 0's chain and the returned event marks the end of unit 1's (the caller orders unit 1's consumers after it)."""
+    def step(self, mf: Tensor, agg: Tensor, gamma: Tensor) -> torch.cuda.Event:
+        """one SepConvGRU update of both units with x = [inp | mf | mf + gamma * agg]; new state in `self.h[u]`.
+        One 4-launch chain per unit: with 84 CTA tiles per unit (640x480: two 60x80 maps) a launch covering both units would be
+        168 CTAs = two waves on 132 SMs per stage, two independent chains of 84-CTA launches keep the SMs filled across the stage
+        boundaries. Unit 0's chain runs on the current stream, unit 1's on a side stream; the returned event marks the end of
+        unit 1's chain, and whatever reads unit 1's state must make its stream wait on it."""
         B, H, W = self.shape
         lib = load_library()
         mf, agg = _dense(mf, GRU_HID, "SepConvGruTC mf"), _dense(agg, GRU_HID, "SepConvGruTC agg")
         if mf.numel() != B * H * W * GRU_HID or agg.numel() != mf.numel():
             raise MacvoB200Error("SepConvGruTC.step: expected (pixels, 128) rows")
-        st = _stream()
+        main = torch.cuda.current_stream()
         _check(lib.macvo_gru_tc_pack_motion(mf.data_ptr(), agg.data_ptr(), _dev(gamma, torch.float32, "gamma").data_ptr(),
-                                            self.x[0].data_ptr(), self.x[1].data_ptr(), B, H, W, st), "macvo_gru_tc_pack_motion")
-        if split_units and self.units == 2:
-            main = torch.cuda.current_stream()
-            fork = torch.cuda.Event()
-            fork.record(main)
-            for u, stream in ((1, self._side), (0, main)):
-                with torch.cuda.stream(stream):
-                    if u == 1:
-                        stream.wait_event(fork)
-                    for o in (0, 1):
-                        for stage in (0, 1):
-                            a = self._unit_args[u, o, stage]
-                            _check(lib.macvo_gru_tc_stage(stage, o, B, H, W, 1, a[0], a[1], a[2], a[3], a[4], a[5], a[6],
-                                                          stream.cuda_stream), "macvo_gru_tc_stage")
-                    if u == 1:
-                        join_ev = torch.cuda.Event()
-                        join_ev.record(stream)
-            LAUNCHES[0] += 9
-            if not join:
-                return join_ev
-            main.wait_event(join_ev)
-            return None
+                                            self.x[0].data_ptr(), self.x[1].data_ptr(), B, H, W, main.cuda_stream),
+               "macvo_gru_tc_pack_motion")
+        fork = torch.cuda.Event()
+        fork.record(main)
+        self._side.wait_event(fork)
+        self._chain(1, self._side)
+        unit1_done = torch.cuda.Event()
+        unit1_done.record(self._side)
+        self._chain(0, main)
+        LAUNCHES[0] += 9
+        return unit1_done
+
+    def _chain(self, unit: int, stream: torch.cuda.Stream) -> None:
+        """the 1x5 pass, then the 5x1 pass, of one unit: stage 0 (z | r) and stage 1 (q + blend) each"""
+        B, H, W = self.shape
+        lib = load_library()
         for o in (0, 1):
             for stage in (0, 1):
-                a = self._args[o, stage]
-                _check(lib.macvo_gru_tc_stage(stage, o, B, H, W, self.units, a[0], a[1], a[2], a[3], a[4], a[5], a[6], st),
+                _check(lib.macvo_gru_tc_stage(stage, o, B, H, W, *self._stage_args[unit, o, stage], stream.cuda_stream),
                        "macvo_gru_tc_stage")
-        LAUNCHES[0] += 5
-        return None
 
 
 def convex_upsample(flow: Tensor, mask_logits: Tensor, scale: float = 1.0) -> Tensor:
@@ -1129,21 +1113,6 @@ def softmax_rows_f16(scores: Tensor) -> Tensor:
     out = torch.empty(x.shape, dtype=torch.float16, device=x.device)
     rc = load_library().macvo_softmax_rows_f16(x.data_ptr(), out.data_ptr(), x.numel() // cols, cols, _stream())
     _check(rc, "macvo_softmax_rows_f16")
-    LAUNCHES[0] += 1
-    return out
-
-
-def query_prep(query: Tensor, ln_weight: Tensor, ln_bias: Tensor, coords: Tensor, freq: Tensor, eps: float = 1e-5) -> Tensor:
-    """LayerNorm_64(query (P,64)) + sine position embedding of coords (B,2,H,W) -> (P,64)  (decoder.py:56-66)"""
-    query = _dense(query, 64, "query_prep query")
-    co = _dev(coords, torch.float32, "query_prep coords")
-    B, _, H, W = co.shape
-    if query.numel() != B * H * W * 64 or freq.numel() != 16:
-        raise MacvoB200Error("query_prep: expects query (B*H*W, 64) and 16 frequencies")
-    out = torch.empty_like(query)
-    rc = load_library().macvo_query_prep(query.data_ptr(), _bias_ptr(ln_weight, 64, "ln weight"), _bias_ptr(ln_bias, 64, "ln bias"),
-                                         co.data_ptr(), _bias_ptr(freq, 16, "freq"), out.data_ptr(), B, H * W, float(eps), _stream())
-    _check(rc, "macvo_query_prep")
     LAUNCHES[0] += 1
     return out
 

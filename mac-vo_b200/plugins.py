@@ -20,7 +20,6 @@ non-CUDA device raises.
 """
 from __future__ import annotations
 
-import os
 from dataclasses import dataclass
 from types import SimpleNamespace
 
@@ -98,13 +97,10 @@ class B200_FlowFormerCovFrontend(IFrontend):
         # the reference frontend enables TF32 tensor cores for the dense layers (Frontend.py:275-277)
         torch.backends.cuda.matmul.allow_tf32 = True
         torch.backends.cudnn.allow_tf32 = True
-        if os.environ.get("MACVO_B200_CUDNN_BENCHMARK") == "1":      # experiment switch: cuDNN autotuning of the conv algorithms
-            torch.backends.cudnn.benchmark = True
         torch.set_float32_matmul_precision("medium")
         self._graph = None
         self._static: dict = {}
         self._score: ops.ScoreBuffers | None = None
-        self.dedup_shared_image = os.environ.get("MACVO_B200_DEDUP", "1") != "0"
 
     @property
     def provide_cov(self) -> tuple[bool, bool]:
@@ -119,7 +115,7 @@ class B200_FlowFormerCovFrontend(IFrontend):
 
     def _run(self, input_A, input_B, bl_fx: float):
         # input_A = [t2.L, t1.L], input_B = [t2.R, t2.L]: B[1] is A[0], which the feature encoder then sees once
-        est_flow, est_cov = self.net.inference(input_A, input_B, shared=(0, 1) if self.dedup_shared_image else None)
+        est_flow, est_cov = self.net.inference(input_A, input_B, shared=(0, 1))
         return self._postprocess(est_flow.float(), est_cov.float(), bl_fx)
 
     def _outputs(self, d: dict, clone: bool):

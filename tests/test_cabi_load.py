@@ -99,7 +99,6 @@ def test_layer_ops_refuse_cpu_tensors(lib):
         lambda: ops.fused_qkv_attention(z(2, 49, 384), 8),
         lambda: ops.latent_pool(z(2, 80, 128), z(8, 128), z(128, 128), z(128, 128), z(128)),
         lambda: ops.add_rows_relu_(z(2, 80, 128), z(80, 128)),
-        lambda: ops.query_prep(z(8, 64), z(64), z(64), z(1, 2, 2, 4), z(16)),
         lambda: ops.gru_gates(z(8, 256), z(8, 512), z(8, 128), z(8, 512)),
         lambda: ops.gru_blend(z(8, 128), z(8, 128), z(8, 512), None),
         lambda: ops.gru_input(z(8, 128), z(8, 128), z(1), [z(8, 512)]),

@@ -130,7 +130,7 @@ def test_gru_fused_kernels(ops):
 
 
 @pytest.mark.parametrize("shape", [(1, 60, 80), (1, 12, 16), (2, 13, 17), (1, 90, 160)])
-def test_sepconv_gru_tensor_cores(ops, shape):
+def test_sepconv_gru_wgmma(ops, shape):
     """csrc/gru_conv_tc.cu (wgmma implicit GEMM, fp16 operands, fp32 state) vs SepConvGRU (core/gru.py:22-43) in float64:
     (a) against the same arithmetic with the convolution inputs / filters rounded to fp16 (what the kernel computes): 1e-3,
     (b) against the unrounded float64 GRU: 4e-3 (fp16 operand rounding, the TF32-class bound of this mode). Two steps, two units,
@@ -166,7 +166,7 @@ def test_sepconv_gru_tensor_cores(ops, shape):
     ref_r, ref_t = [to_map(h) for h in h0], [to_map(h) for h in h0]
     for it in range(2):
         mf, agg = rnd(P, 128).relu(), rnd(P, 128)
-        gru.step(mf, agg, gamma, split_units=(it == 1))         # second step: one launch chain per unit on two streams
+        torch.cuda.current_stream().wait_event(gru.step(mf, agg, gamma))     # unit 1's chain runs on a side stream
         xs = torch.cat([inp, mf, mf + gamma * agg], 1)
         for u in range(2):
             # the fp16 rounding of x happens on the fp32 values the pack kernel forms
@@ -310,21 +310,6 @@ def test_lookup_rows_equals_lookup_map(ops):
     b = ops.corr_lookup(cm.to(DEV), co.to(DEV), rows=True)
     assert b.shape == (2 * 12 * 16, 81)
     assert torch.equal(a.permute(0, 2, 3, 1).reshape(-1, 81), b)          # same arithmetic, other layout: bit-exact
-
-
-def test_query_prep(ops):
-    """LayerNorm(query) + LinearPositionEmbeddingSine(coords) (decoder.py:56-66, attention.py:71-101) vs torch ops"""
-    from macvo_b200.flowformer_cov import sine_embed
-    g = torch.Generator().manual_seed(5)
-    B, H, W = 2, 9, 13
-    P = B * H * W
-    query = torch.randn(P, 64, generator=g).to(DEV) * 2
-    w, b = torch.randn(64, generator=g).to(DEV), torch.randn(64, generator=g).to(DEV)
-    coords = (torch.rand(B, 2, H, W, generator=g) * 90 - 5).to(DEV)
-    freq = torch.arange(16, device=DEV, dtype=torch.float32) * (1 / 200) * torch.pi
-    ref = F.layer_norm(query, (64,), w, b) + sine_embed(coords.permute(0, 2, 3, 1).reshape(P, 2), 64)
-    got = ops.query_prep(query, w, b, coords, freq)
-    torch.testing.assert_close(got, ref, rtol=1e-5, atol=2e-5)
 
 
 @pytest.mark.parametrize("tf32", [False, True])

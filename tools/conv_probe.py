@@ -1,4 +1,4 @@
-"""Event trace + graph timing of one tensor-core (wgmma) convolution (csrc/conv_tc.cu) at the decoder's shapes (B = 2, 60 x 80)."""
+"""Graph timing of one tensor-core (wgmma) convolution (csrc/conv_tc.cu) at the decoder's shapes (B = 2, 60 x 80)."""
 import json
 import os
 import sys
@@ -11,7 +11,6 @@ DEV = "cuda:0"
 torch.backends.cudnn.allow_tf32 = True
 B, H, W = 2, 60, 80
 shape = (B, H, W)
-lib = ops.load_library()
 g = torch.Generator().manual_seed(0)
 flush = torch.empty(256 << 20, dtype=torch.uint8, device=DEV)
 
@@ -49,15 +48,4 @@ for cin, cout, k in ((256, 192, 3), (256, 126, 3), (128, 256, 3), (192, 256, 1),
     res = {"conv": [cin, cout, k],
            "tc_us": graphed(lambda: ops.conv_tc(rows, wp, bp, n, k, True, shape, out16=out16)),
            "cudnn_relu_us": graphed(lambda: torch.cudnn_convolution_relu(xl, wl, b, (1, 1), (k // 2, k // 2), (1, 1), 1))}
-    tr = torch.zeros(3 * 64, dtype=torch.int64, device=DEV)
-    lib.macvo_conv_tc_set_trace(tr.data_ptr())
-    ops.conv_tc(rows, wp, bp, n, k, True, shape, out16=out16)
-    torch.cuda.synchronize()
-    lib.macvo_conv_tc_set_trace(None)
-    t = tr.cpu().view(3, 64)
-    t0 = int(t[2, 0])
-    rel = lambda row: [int(v) - t0 for v in row if int(v) != 0]
     print(json.dumps(res))
-    print("  epilogue warp (start, griddep passed, tfull, stores done, exit):", rel(t[2]))
-    print("  producer (after griddep wait, then every A issue):", rel(t[0])[:16])
-    print("  MMA step starts:", rel(t[1])[:40])

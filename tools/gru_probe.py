@@ -73,33 +73,15 @@ def graphed(fn, reps=10):
     return timed(gr.replay, 20) / reps
 
 
-out = {"shape": [B, H, W], "tc_step_us": timed(lambda: gru.step(mf, agg, gamma)), "cudnn_glue_step_us": timed(old_step),
-       "tc_step_graph_us": graphed(lambda: gru.step(mf, agg, gamma)), "cudnn_glue_step_graph_us": graphed(old_step)}
+def tc_step():
+    torch.cuda.current_stream().wait_event(gru.step(mf, agg, gamma))
+
+
+out = {"shape": [B, H, W], "tc_step_us": timed(tc_step), "cudnn_glue_step_us": timed(old_step),
+       "tc_step_graph_us": graphed(tc_step), "cudnn_glue_step_graph_us": graphed(old_step)}
 lib = ops.load_library()
-st = torch.cuda.current_stream().cuda_stream
-for o in (0, 1):
-    for stage in (0, 1):
-        a = gru._args[o, stage]
-        out[f"stage{stage}_pass{o}_graph_us"] = graphed(lambda: lib.macvo_gru_tc_stage(stage, o, B, H, W, 2, a[0], a[1], a[2], a[3], a[4], a[5], a[6],
-                                                                                       torch.cuda.current_stream().cuda_stream))
 out["pack_motion_graph_us"] = graphed(lambda: lib.macvo_gru_tc_pack_motion(mf.data_ptr(), agg.data_ptr(), gamma.data_ptr(), gru.x[0].data_ptr(),
                                                                            gru.x[1].data_ptr(), B, H, W, torch.cuda.current_stream().cuda_stream))
 flops = 2 * 2 * P * 384 * 2560 * 2          # both passes, both units
 out["tc_tflops"] = flops / out["tc_step_graph_us"] / 1e6
 print(json.dumps(out))
-
-# event trace of the first CTA (globaltimer, ns relative to kernel start): producer B issues | MMA steps | epilogue phases
-tr = torch.zeros(3 * 64, dtype=torch.int64, device=DEV)
-for o, stage in ((0, 0), (0, 1)):
-    a = gru._args[o, stage]
-    tr.zero_()
-    lib.macvo_gru_tc_set_trace(tr.data_ptr())
-    lib.macvo_gru_tc_stage(stage, o, B, H, W, 2, a[0], a[1], a[2], a[3], a[4], a[5], a[6], torch.cuda.current_stream().cuda_stream)
-    torch.cuda.synchronize()
-    lib.macvo_gru_tc_set_trace(None)
-    t = tr.cpu().view(3, 64)
-    t0 = int(t[2, 0])
-    rel = lambda row: [int(v) - t0 for v in row if int(v) != 0]
-    print(f"trace stage {stage}: epilogue-warp events (start, prologue done, pre-wait, tfull, epilogue done, exit) =", rel(t[2]))
-    print("  producer B-slot issue times:", rel(t[0]))
-    print("  MMA step start times:", rel(t[1]))
