@@ -229,7 +229,10 @@ int macvo_pgo_solve_graph(int graph_type, const double* pos_Tw, const double* kp
  * stats[7] = 1 when a rank-deficient covariance block received its pseudo-inverse weight. */
 int macvo_pgo_solve_counted(const double* pos_Tw, const double* kp2_uv, const double* kp2_disp, const double* uv_cov,
                             const double* disp_cov, int k_capacity, const int* k_dev, int min_k, const double* intr,
-                            double* pose_io, const macvo_pgo_params_t* params, double* stats, void* stream);
+                            double* pose_io, const macvo_pgo_params_t* params, double* stats, void* stream,
+                            int graph_type, const double* pc_obs, const double* obs_cov, const double* pts_cov);
+/* graph_type / pc_obs / obs_cov / pts_cov as in macvo_pgo_solve_graph (0 / NULL: "disp", as before); for MACVO_PGO_ICP
+ * they are the points_Tc / obs2_covTc / cov_Tw sections of an extended macvo_observe_pack buffer. */
 
 /* Multi-GPU solve (BASELINE config 4; SURVEY.md §8e): the K residual blocks are sharded across `world` ranks (one process
  * per GPU), every rank launches this with ITS shard and the same pose_io / params; the all-reduce of the 55-double
@@ -403,14 +406,35 @@ int macvo_convex_upsample(const float* flow, const float* mask_nhwc, float* out,
 /* CovarianceSanityFilter.filter (Module/OutlierFilter.py:91-100) on device-resident (k,3,3) float64 covariances:
  * good[i] = 1 iff neither matrix of observation i holds a NaN / Inf. */
 int macvo_cov_sanity_filter(const double* obs1_cov, const double* obs2_cov, int k, uint8_t* good, void* stream);
+/* Optional extension of macvo_observe_pack (HOST struct; NULL = sanity filter only, the layout above): the other two
+ * observation filters of FilterCompose (Module/OutlierFilter.py:106-141) and the columns of the "icp" pose graph.
+ * Per in-bound row the kernel also gathers pixel2_d = depth1 at the truncated kp1, pixel1_d_cov = depth_cov0 at kp0 and
+ * pixel2_d_cov = depth_cov1 at kp1 (-1, the reference's placeholder, where the map is NULL). fp32 throughout:
+ *   simple_depth  drop a row when d < min_depth or d > max_depth on either frame (NaN depth passes);
+ *   front_of_cam  keep a row when d - 2 sqrt(d_cov) > 0 on both frames (NaN / negative d_cov drops it), unless ANY
+ *                 in-bound row has pixel1_d_cov == -1: then this filter passes every row;
+ *   icp           also pack pixel2_d, pixel1_d_cov, pixel2_d_cov, points_Tc = pixel2point_NED(pixel2_uv, pixel2_d, K1)
+ *                 (fp32, widened) and cov_Tw = R obs1_covTc R^T (float64; R = rotation matrix of prev_pose rounded to
+ *                 fp32, computed in fp32, widened) for the kept rows, AFTER the header (every offset above stays):
+ *   [31c+4,32c+4) pixel2_d | [32c+4,33c+4) pixel1_d_cov | [33c+4,34c+4) pixel2_d_cov | [34c+4,37c+4) points_Tc (c,3)
+ *   [37c+4,46c+4) cov_Tw (c,3,3)        -> `packed` must hold macvo_observe_packed_doubles(capacity, 1) = 46c + 4 doubles.
+ * macvo_observe_packed_doubles(capacity, 0) = 31c + 4. */
+typedef struct {
+    const float* depth_cov0; /* (h,w) device, or NULL */
+    const float* depth_cov1; /* (h,w) device, or NULL */
+    int simple_depth;
+    float min_depth, max_depth;
+    int front_of_cam;
+    int icp;
+} macvo_observe_ext_t;
 size_t macvo_observe_workspace_bytes(int capacity);
-size_t macvo_observe_packed_doubles(int capacity);
+size_t macvo_observe_packed_doubles(int capacity, int extended);
 int macvo_observe_pack(const int64_t* kp0_uv, int k, int capacity, const float* flow, const float* match_cov,
                        const float* depth0, const float* depth1, const float* disparity1, const float* disp_unc1,
                        int h, int w, int edge_width, const float* intr0, const float* intr1, int kernel_size,
                        float min_flow_cov, float min_depth_cov, float match_cov_default, const double* prev_pose,
                        double* next_pose, double* packed, int* n_obs, int* status, void* workspace,
-                       size_t workspace_bytes, void* stream);
+                       size_t workspace_bytes, void* stream, const macvo_observe_ext_t* ext);
 
 /* ------------------------------------------------------------------------------------------------
  * (f2) decoder token path of one refinement iteration as one kernel — replaces flow_token_encoder (decoder.py:112-116),

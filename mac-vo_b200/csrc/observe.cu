@@ -33,11 +33,19 @@ struct ObserveArgs {
     float min_flow_var, match_cov_default;
     const double* prev_pose;       // (7) [t, q_xyzw] optimised pose of frame 0 (device, float64)
     double* next_pose;             // (7) receives the motion-model prediction for frame 1 (= prev pose, fp32-rounded)
+    // macvo_observe_ext_t (ext == 0: none of this is read or written)
+    int ext, simple_depth, front_of_cam;
+    float min_depth, max_depth;
+    const float* depth_cov0;       // (h,w) or nullptr (-1 placeholder)
+    const float* depth_cov1;
+    float* rex;                    // (k, REX) extension records
 };
 
 // record slot (floats): 0 keep | 1,2 kp1 uv | 3 depth0 | 4 disp1 | 5 disp_unc1 | 6..8 uv cov (clamped) | 9..11 pos_Tw |
 //                       12..17 cov0 (6 unique) | 18..23 cov1 (6 unique) | 24 inbound
 constexpr int REC = 25;
+// extension record (ext only): 0 pixel2_d | 1 pixel1_d_cov | 2 pixel2_d_cov | 3 LikelyFrontOfCam verdict | 4..6 points_Tc
+constexpr int REX = 7;
 
 __device__ __forceinline__ bool bad6(const float* s) {
     bool b = false;
@@ -89,7 +97,25 @@ observe_kernel(ObserveArgs A, float* __restrict__ rec, int* __restrict__ status)
     if (lane != 0) return;
     if (oob) atomicOr(status, 1);                // status is a bitmask: both conditions may occur in one call
     // CovarianceSanityFilter: drop observations with NaN / Inf covariance on either frame
-    const bool keep = !(bad6(c0) || bad6(c1));
+    bool keep = !(bad6(c0) || bad6(c1));
+    if (A.ext) {
+        // Module/OutlierFilter.py:106-141 in fp32 on the MatchObs columns (MACVO.py:205-248 gathers)
+        const float d1 = A.depth1[p1];
+        const float dc0 = A.depth_cov0 ? A.depth_cov0[p0] : -1.f, dc1 = A.depth_cov1 ? A.depth_cov1[p1] : -1.f;
+        // SimpleDepthFilter: ordered comparisons are false for NaN, so a NaN depth passes
+        if (A.simple_depth)
+            keep &= !(d0 < A.min_depth || d0 > A.max_depth || d1 < A.min_depth || d1 > A.max_depth);
+        // LikelyFrontOfCamFilter: d - sqrt(d_cov) * 2 > 0 on both frames; pack_kernel applies it unless a placeholder
+        // pixel1_d_cov == -1 exists among the in-bound rows
+        const bool front = __fsub_rn(d0, __fmul_rn(__fsqrt_rn(dc0), 2.f)) > 0.f &&
+                           __fsub_rn(d1, __fmul_rn(__fsqrt_rn(dc1), 2.f)) > 0.f;
+        float* x = A.rex + (long long)i * REX;
+        x[0] = d1; x[1] = dc0; x[2] = dc1; x[3] = front ? 1.f : 0.f;
+        // ICP_TwoframePGO's points_Tc = pixel2point_NED(pixel2_uv, pixel2_d, K1) (Graphs.py:49-51)
+        x[4] = d1;
+        x[5] = __fmul_rn(__fdiv_rn(__fsub_rn(u1, A.P1.cx), A.P1.fx), d1);
+        x[6] = __fmul_rn(__fdiv_rn(__fsub_rn(v1, A.P1.cy), A.P1.fy), d1);
+    }
     // pixel2point_NED (Utility/Point.py:15-17): [d, (u - cx) / fx * d, (v - cy) / fy * d]
     const float px = d0;
     const float py = __fmul_rn(__fdiv_rn(__fsub_rn((float)u0, A.P0.cx), A.P0.fx), d0);
@@ -114,23 +140,59 @@ observe_kernel(ObserveArgs A, float* __restrict__ rec, int* __restrict__ status)
     r[24] = 1.f;
 }
 
+struct PackExt {
+    int on, front_of_cam, icp;
+    const float* rex;
+    const double* prev_pose;
+};
+
 // packed float64 buffer, sections sized by the CAPACITY cap (fixed pointers for the LM kernel):
 //   [0,3c) pos_Tw | [3c,5c) kp2 uv | [5c,6c) kp2 disp | [6c,9c) uv cov | [9c,10c) disp cov          <- pgo.cu inputs
 //   [10c,19c) obs1_covTc (c,3,3) | [19c,28c) obs2_covTc (c,3,3) | [28c,30c) pixel1_uv | [30c,31c) pixel1_d
 //   [31c,31c+4) header: n_obs, n_inbound, k, status
+// with the icp extension, after the header (E = 31c+4):
+//   [E,E+c) pixel2_d | [E+c,E+2c) pixel1_d_cov | [E+2c,E+3c) pixel2_d_cov | [E+3c,E+6c) points_Tc | [E+6c,E+15c) cov_Tw
 __global__ void __launch_bounds__(1024)
 pack_kernel(const float* __restrict__ rec, const int64_t* __restrict__ kp0, int k, int cap, double* __restrict__ out,
-            int* __restrict__ n_obs, const int* __restrict__ status) {
+            int* __restrict__ n_obs, const int* __restrict__ status, PackExt X) {
     __shared__ int s_warp[32];
     __shared__ int s_base, s_inb;
+    __shared__ double s_R[9];
     if (threadIdx.x == 0) { s_base = 0; s_inb = 0; }
-    __syncthreads();
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const long long c = cap;
+    bool front_all = false;
+    if (X.on) {
+        if (X.icp && threadIdx.x == 0) {
+            // pp.SE3(fp32 pose).rotation().matrix() in fp32, then .to(torch.float64) (MACVO.py:274-275)
+            const float qx = (float)X.prev_pose[3], qy = (float)X.prev_pose[4], qz = (float)X.prev_pose[5],
+                        qw = (float)X.prev_pose[6];
+            const float xx = __fmul_rn(qx, qx), yy = __fmul_rn(qy, qy), zz = __fmul_rn(qz, qz);
+            const float xy = __fmul_rn(qx, qy), xz = __fmul_rn(qx, qz), yz = __fmul_rn(qy, qz);
+            const float xw = __fmul_rn(qx, qw), yw = __fmul_rn(qy, qw), zw = __fmul_rn(qz, qw);
+            s_R[0] = __fsub_rn(1.f, __fmul_rn(2.f, __fadd_rn(yy, zz)));
+            s_R[1] = __fmul_rn(2.f, __fsub_rn(xy, zw));
+            s_R[2] = __fmul_rn(2.f, __fadd_rn(xz, yw));
+            s_R[3] = __fmul_rn(2.f, __fadd_rn(xy, zw));
+            s_R[4] = __fsub_rn(1.f, __fmul_rn(2.f, __fadd_rn(xx, zz)));
+            s_R[5] = __fmul_rn(2.f, __fsub_rn(yz, xw));
+            s_R[6] = __fmul_rn(2.f, __fsub_rn(xz, yw));
+            s_R[7] = __fmul_rn(2.f, __fadd_rn(yz, xw));
+            s_R[8] = __fsub_rn(1.f, __fmul_rn(2.f, __fadd_rn(xx, yy)));
+        }
+        // LikelyFrontOfCamFilter passes every row when any in-bound row holds the -1 placeholder (OutlierFilter.py:130-133)
+        int ph = 0;
+        if (X.front_of_cam)
+            for (int i = threadIdx.x; i < k; i += 1024)
+                ph |= rec[(long long)i * REC + 24] != 0.f && X.rex[(long long)i * REX + 1] == -1.f;
+        front_all = __syncthreads_or(ph) != 0 || !X.front_of_cam;
+    }
+    __syncthreads();
     for (int start = 0; start < k; start += 1024) {
         const int i = start + threadIdx.x;
         const float* r = rec + (long long)i * REC;
-        const bool keep = i < k && r[0] != 0.f;
+        const float* x = X.rex + (long long)i * REX;
+        const bool keep = i < k && r[0] != 0.f && (!X.on || front_all || x[3] != 0.f);
         const bool inb = i < k && r[24] != 0.f;
         const unsigned bal = __ballot_sync(0xffffffffu, keep);
         const unsigned bal_in = __ballot_sync(0xffffffffu, inb);
@@ -149,6 +211,25 @@ pack_kernel(const float* __restrict__ rec, const int64_t* __restrict__ kp0, int 
             macvo::store_cov9(out + 19 * c + 9LL * j, r + 18);
             out[28 * c + 2 * j] = (double)kp0[2 * i]; out[28 * c + 2 * j + 1] = (double)kp0[2 * i + 1];
             out[30 * c + j] = r[3];
+            if (X.icp) {
+                double* e = out + 31 * c + 4;
+                e[j] = x[0]; e[c + j] = x[1]; e[2 * c + j] = x[2];
+                e[3 * c + 3 * j] = x[4]; e[3 * c + 3 * j + 1] = x[5]; e[3 * c + 3 * j + 2] = x[6];
+                // cov_Tw = R obs1_covTc R^T in float64 (torch.bmm(torch.bmm(R, cov), R^T), MACVO.py:280)
+                double C[9], RC[9];
+                macvo::store_cov9(C, r + 12);
+#pragma unroll
+                for (int a = 0; a < 3; ++a)
+#pragma unroll
+                    for (int b = 0; b < 3; ++b)
+                        RC[3 * a + b] = s_R[3 * a] * C[b] + s_R[3 * a + 1] * C[3 + b] + s_R[3 * a + 2] * C[6 + b];
+                double* o = e + 6 * c + 9LL * j;
+#pragma unroll
+                for (int a = 0; a < 3; ++a)
+#pragma unroll
+                    for (int b = 0; b < 3; ++b)
+                        o[3 * a + b] = RC[3 * a] * s_R[3 * b] + RC[3 * a + 1] * s_R[3 * b + 1] + RC[3 * a + 2] * s_R[3 * b + 2];
+            }
         }
         __syncthreads();
         if (threadIdx.x == 0) s_base += tot;
@@ -183,17 +264,20 @@ extern "C" int macvo_cov_sanity_filter(const double* obs1_cov, const double* obs
 }
 
 extern "C" size_t macvo_observe_workspace_bytes(int capacity) {
-    return (size_t)capacity * REC * sizeof(float);
+    return (size_t)capacity * (REC + REX) * sizeof(float);
 }
 
-extern "C" size_t macvo_observe_packed_doubles(int capacity) { return (size_t)31 * capacity + 4; }
+extern "C" size_t macvo_observe_packed_doubles(int capacity, int extended) {
+    return (size_t)(extended ? 46 : 31) * capacity + 4;
+}
 
 extern "C" int macvo_observe_pack(const int64_t* kp0_uv, int k, int capacity, const float* flow, const float* match_cov,
                                   const float* depth0, const float* depth1, const float* disparity1,
                                   const float* disp_unc1, int h, int w, int edge_width, const float* intr0,
                                   const float* intr1, int kernel_size, float min_flow_cov, float min_depth_cov,
                                   float match_cov_default, const double* prev_pose, double* next_pose, double* packed,
-                                  int* n_obs, int* status, void* workspace, size_t workspace_bytes, void* stream) {
+                                  int* n_obs, int* status, void* workspace, size_t workspace_bytes, void* stream,
+                                  const macvo_observe_ext_t* ext) {
     if (k < 0 || capacity < 1 || k > capacity || h <= 0 || w <= 0 || edge_width <= 0 || kernel_size < 1 ||
         (kernel_size & 1) == 0 || kernel_size > 31)
         return MACVO_E_ARG;
@@ -201,6 +285,7 @@ extern "C" int macvo_observe_pack(const int64_t* kp0_uv, int k, int capacity, co
         !next_pose || !packed || !n_obs || !status || !workspace || (k > 0 && !kp0_uv))
         return MACVO_E_ARG;
     if (workspace_bytes < macvo_observe_workspace_bytes(capacity)) return MACVO_E_WORKSPACE;
+    if (ext && ext->simple_depth && !(ext->min_depth <= ext->max_depth)) return MACVO_E_ARG;
     ObserveArgs A;
     A.kp0 = kp0_uv; A.k = k; A.flow = flow; A.match_cov = match_cov; A.depth0 = depth0; A.depth1 = depth1;
     A.disparity1 = disparity1; A.disp_unc1 = disp_unc1; A.h = h; A.w = w; A.edge = edge_width;
@@ -209,11 +294,17 @@ extern "C" int macvo_observe_pack(const int64_t* kp0_uv, int k, int capacity, co
     A.min_flow_var = min_flow_cov * min_flow_cov;
     A.match_cov_default = match_cov_default;
     A.prev_pose = prev_pose; A.next_pose = next_pose;
-    cudaStream_t st = as_stream(stream);
     float* rec = static_cast<float*>(workspace);
+    A.ext = ext != nullptr;
+    A.simple_depth = ext && ext->simple_depth; A.front_of_cam = ext && ext->front_of_cam;
+    A.min_depth = ext ? ext->min_depth : 0.f; A.max_depth = ext ? ext->max_depth : 0.f;
+    A.depth_cov0 = ext ? ext->depth_cov0 : nullptr; A.depth_cov1 = ext ? ext->depth_cov1 : nullptr;
+    A.rex = rec + (size_t)capacity * REC;
+    PackExt X{A.ext, A.front_of_cam, ext && ext->icp, A.rex, prev_pose};
+    cudaStream_t st = as_stream(stream);
     observe_kernel<<<max(1, ceil_div(k * 32, 128)), 128, 0, st>>>(A, rec, status);
     MACVO_LAUNCH_CHECK();
-    pack_kernel<<<1, 1024, 0, st>>>(rec, kp0_uv, k, capacity, packed, n_obs, status);
+    pack_kernel<<<1, 1024, 0, st>>>(rec, kp0_uv, k, capacity, packed, n_obs, status, X);
     MACVO_LAUNCH_CHECK();
     return MACVO_OK;
 }

@@ -635,10 +635,12 @@ extern "C" int macvo_pgo_solve_graph(int graph_type, const double* pos_Tw, const
 extern "C" int macvo_pgo_solve_counted(const double* pos_Tw, const double* kp2_uv, const double* kp2_disp,
                                        const double* uv_cov, const double* disp_cov, int k_capacity, const int* k_dev,
                                        int min_k, const double* intr, double* pose_io,
-                                       const macvo_pgo_params_t* params, double* stats, void* stream) {
+                                       const macvo_pgo_params_t* params, double* stats, void* stream, int graph_type,
+                                       const double* pc_obs, const double* obs_cov, const double* pts_cov) {
     if (!k_dev || min_k < 0) return MACVO_E_ARG;
+    // every graph type's loops run over P.k = min(*k_dev, k_capacity): no block at or past the survivor count is read
     return pgo_solve_impl(pos_Tw, kp2_uv, kp2_disp, uv_cov, disp_cov, k_capacity, k_dev, min_k, intr, pose_io, params,
-                          stats, stream);
+                          stats, stream, nullptr, 1, 0, 0, GraphExtra{graph_type, pc_obs, obs_cov, pts_cov});
 }
 
 // ---- multi-GPU: sharded residual blocks, all-reduce fused into the persistent kernel over peer memory ---------------------

@@ -37,6 +37,11 @@ class _ScoreT(C.Structure):
                 ("cand_vals2", C.c_void_p)]
 
 
+class _ObserveExt(C.Structure):
+    _fields_ = [("depth_cov0", C.c_void_p), ("depth_cov1", C.c_void_p), ("simple_depth", C.c_int),
+                ("min_depth", C.c_float), ("max_depth", C.c_float), ("front_of_cam", C.c_int), ("icp", C.c_int)]
+
+
 class _PgoParams(C.Structure):
     _fields_ = [("max_steps", C.c_int), ("patience", C.c_int), ("max_reject", C.c_int), ("cluster", C.c_int),
                 ("decreasing", C.c_double), ("huber_delta", C.c_double), ("radius", C.c_double),
@@ -68,14 +73,15 @@ EXPORTS = {
     "macvo_pgo_solve_graph": (C.c_int, [C.c_int] + [C.c_void_p] * 8 + [C.c_int] + [C.c_void_p] * 2 + [C.POINTER(_PgoParams)]
                               + [C.c_void_p] * 2),
     "macvo_pgo_solve_counted": (C.c_int, [C.c_void_p] * 5 + [C.c_int, C.c_void_p, C.c_int] + [C.c_void_p] * 2
-                                + [C.POINTER(_PgoParams)] + [C.c_void_p] * 2),
+                                + [C.POINTER(_PgoParams)] + [C.c_void_p] * 2 + [C.c_int] + [C.c_void_p] * 3),
     "macvo_motion_interpolate_workspace_bytes": (C.c_size_t, [C.c_int]),
     "macvo_motion_interpolate": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     "macvo_cov_sanity_filter": (C.c_int, [C.c_void_p] * 2 + [C.c_int] + [C.c_void_p] * 2),
     "macvo_observe_workspace_bytes": (C.c_size_t, [C.c_int]),
-    "macvo_observe_packed_doubles": (C.c_size_t, [C.c_int]),
+    "macvo_observe_packed_doubles": (C.c_size_t, [C.c_int, C.c_int]),
     "macvo_observe_pack": (C.c_int, [C.c_void_p, C.c_int, C.c_int] + [C.c_void_p] * 6 + [C.c_int] * 3 + [C.c_void_p] * 2
-                           + [C.c_int] + [C.c_float] * 3 + [C.c_void_p] * 6 + [C.c_size_t, C.c_void_p]),
+                           + [C.c_int] + [C.c_float] * 3 + [C.c_void_p] * 6 + [C.c_size_t, C.c_void_p]
+                           + [C.POINTER(_ObserveExt)]),
     "macvo_pgo_exchange_bytes": (C.c_size_t, [C.c_int]),
     "macvo_p2p_alloc": (C.c_int, [C.c_size_t, C.POINTER(C.c_void_p), C.c_char_p]),
     "macvo_p2p_open": (C.c_int, [C.c_char_p, C.POINTER(C.c_void_p)]),
@@ -578,12 +584,14 @@ def pgo_accumulate(pos_Tw: Tensor, kp2_uv: Tensor, kp2_disp: Tensor, uv_cov: Ten
 # (f3) device-side observation building / sanity filter / MatchObs packing + counted PGO solve
 # ------------------------------------------------------------------------------------------------
 class ObservationBuffers:
-    """Device + pinned-host buffers of one frame's observations (layout: include/macvo_b200.h, macvo_observe_pack)."""
+    """Device + pinned-host buffers of one frame's observations (layout: include/macvo_b200.h, macvo_observe_pack).
+    `extended`: room for the columns the "icp" graph reads (pixel2_d .. cov_Tw, after the header)."""
 
-    def __init__(self, capacity: int, device):
+    def __init__(self, capacity: int, device, extended: bool = False):
         lib = load_library()
         self.capacity = int(capacity)
-        self.n_doubles = int(lib.macvo_observe_packed_doubles(self.capacity))
+        self.extended = bool(extended)
+        self.n_doubles = int(lib.macvo_observe_packed_doubles(self.capacity, int(self.extended)))
         self.packed = torch.zeros((self.n_doubles,), dtype=torch.float64, device=device)
         self.n_obs = torch.zeros((1,), dtype=torch.int32, device=device)
         self.status = torch.zeros((1,), dtype=torch.int32, device=device)
@@ -598,7 +606,14 @@ class ObservationBuffers:
                          "pixel2_uv_cov": (6 * c, 9 * c, (c, 3)), "pixel2_disp_cov": (9 * c, 10 * c, (c,)),
                          "obs1_covTc": (10 * c, 19 * c, (c, 3, 3)), "obs2_covTc": (19 * c, 28 * c, (c, 3, 3)),
                          "pixel1_uv": (28 * c, 30 * c, (c, 2)), "pixel1_d": (30 * c, 31 * c, (c,)),
-                         "header": (31 * c, 31 * c + 4, (4,))}[name]
+                         "header": (31 * c, 31 * c + 4, (4,))}.get(name, (None, None, None))
+        if lo is None and self.extended:
+            e = 31 * c + 4
+            lo, hi, shape = {"pixel2_d": (e, e + c, (c,)), "pixel1_d_cov": (e + c, e + 2 * c, (c,)),
+                             "pixel2_d_cov": (e + 2 * c, e + 3 * c, (c,)), "points_Tc": (e + 3 * c, e + 6 * c, (c, 3)),
+                             "cov_Tw": (e + 6 * c, e + 15 * c, (c, 3, 3))}.get(name, (None, None, None))
+        if lo is None:
+            raise KeyError(f"ObservationBuffers: no section {name!r}" + ("" if self.extended else " (not extended)"))
         return (self.host if host else self.packed)[lo:hi].view(shape)
 
     def download_async(self) -> None:
@@ -641,8 +656,12 @@ def cov_sanity_filter(obs1_cov: Tensor, obs2_cov: Tensor) -> Tensor:
 def observe_pack(buf: ObservationBuffers, kp0_uv: Tensor, flow: Tensor, match_cov: Tensor, depth0: Tensor, depth1: Tensor,
                  disparity1: Tensor, disp_unc1: Tensor, edge_width: int, intr0, intr1, prev_pose: Tensor, next_pose: Tensor,
                  kernel_size: int = 31, min_flow_cov: float = 0.25, min_depth_cov: float = 0.05,
-                 match_cov_default: float = 0.25) -> None:
-    """Odometry/MACVO.py:198-283 for the two-frame graph as two launches (csrc/observe.cu); everything stays on the device."""
+                 match_cov_default: float = 0.25, ext: dict | None = None) -> None:
+    """Odometry/MACVO.py:198-283 for the two-frame graph as two launches (csrc/observe.cu); everything stays on the device.
+
+    ext (None: CovarianceSanityFilter only) = macvo_observe_ext_t as a dict: depth_cov0 / depth_cov1 ((1,1,H,W) fp32 CUDA
+    or None), simple_depth (bool), min_depth / max_depth (floats, rounded to fp32 like the reference's comparisons),
+    front_of_cam (bool), icp (bool: pack the "icp" graph's columns; needs an extended buffer)."""
     lib = load_library()
     kp = _dev(kp0_uv, torch.int64, "observe_pack kp0_uv")
     k = kp.shape[0]
@@ -659,28 +678,49 @@ def observe_pack(buf: ObservationBuffers, kp0_uv: Tensor, flow: Tensor, match_co
         raise MacvoB200Error("observe_pack: next_pose must be a contiguous (7,) float64 CUDA tensor")
     i0 = (C.c_float * 4)(*[float(v) for v in intr0])
     i1 = (C.c_float * 4)(*[float(v) for v in intr1])
+    xs = None
+    if ext is not None:
+        unknown = set(ext) - {"depth_cov0", "depth_cov1", "simple_depth", "min_depth", "max_depth", "front_of_cam", "icp"}
+        if unknown:
+            raise MacvoB200Error(f"observe_pack: unknown ext keys {sorted(unknown)}")
+        if ext.get("icp") and not buf.extended:
+            raise MacvoB200Error("observe_pack: the icp columns need ObservationBuffers(..., extended=True)")
+        dc = [None if ext.get(n) is None else _dev(ext[n], torch.float32, f"observe_pack {n}") for n in ("depth_cov0", "depth_cov1")]
+        if any(m is not None and m.numel() != H * W for m in dc):
+            raise MacvoB200Error("observe_pack: depth_cov0 / depth_cov1 must be (1,1,H,W) maps")
+        xs = _ObserveExt(None if dc[0] is None else dc[0].data_ptr(), None if dc[1] is None else dc[1].data_ptr(),
+                         int(bool(ext.get("simple_depth"))), float(ext.get("min_depth", 0.0)), float(ext.get("max_depth", 0.0)),
+                         int(bool(ext.get("front_of_cam"))), int(bool(ext.get("icp"))))
     buf.status.zero_()
     rc = lib.macvo_observe_pack(kp.data_ptr() if k else None, k, buf.capacity, fl.data_ptr(), mc.data_ptr(),
                                 *(m.data_ptr() for m in maps), H, W, int(edge_width), C.cast(i0, C.c_void_p),
                                 C.cast(i1, C.c_void_p), int(kernel_size), float(min_flow_cov), float(min_depth_cov),
                                 float(match_cov_default), pp.data_ptr(), next_pose.data_ptr(), buf.packed.data_ptr(),
-                                buf.n_obs.data_ptr(), buf.status.data_ptr(), buf.ws.data_ptr(), buf.ws_bytes, _stream())
+                                buf.n_obs.data_ptr(), buf.status.data_ptr(), buf.ws.data_ptr(), buf.ws_bytes, _stream(),
+                                None if xs is None else C.byref(xs))
     _check(rc, "macvo_observe_pack")
     LAUNCHES[0] += 2
 
 
 def pgo_solve_counted(buf: ObservationBuffers, intr: tuple[float, float, float, float, float], pose_io: Tensor,
-                      stats: Tensor, min_k: int = 10, cluster: int = 0, **kw) -> None:
+                      stats: Tensor, min_k: int = 10, cluster: int = 0, graph_type: str = "disp", **kw) -> None:
     """LM solve on the packed observation arrays, block count read from buf.n_obs on the device; pose_io (7,) float64
-    CUDA holds the initial pose and receives the result (untouched when fewer than min_k observations survive)."""
+    CUDA holds the initial pose and receives the result (untouched when fewer than min_k observations survive).
+    graph_type "icp" reads points_Tc / obs2_covTc / cov_Tw of an extended buffer that observe_pack filled with icp on."""
     lib = load_library()
     c = buf.capacity
     base = buf.packed.data_ptr()
+    gt = PGO_GRAPH_TYPES[graph_type]
+    icp = (None, None, None)
+    if gt == PGO_GRAPH_TYPES["icp"]:
+        if not buf.extended:
+            raise MacvoB200Error("pgo_solve_counted: graph type 'icp' needs ObservationBuffers(..., extended=True)")
+        icp = tuple(buf.section(n).data_ptr() for n in ("points_Tc", "obs2_covTc", "cov_Tw"))
     intr_c = (C.c_double * 5)(*[float(v) for v in intr])
     prm = _pgo_params(cluster=cluster, **kw)       # 0: cluster size chosen from the capacity
     rc = lib.macvo_pgo_solve_counted(base, base + 8 * 3 * c, base + 8 * 5 * c, base + 8 * 6 * c, base + 8 * 9 * c, c,
                                      buf.n_obs.data_ptr(), int(min_k), C.cast(intr_c, C.c_void_p), pose_io.data_ptr(),
-                                     C.byref(prm), stats.data_ptr(), _stream())
+                                     C.byref(prm), stats.data_ptr(), _stream(), gt, *icp)
     _check(rc, "macvo_pgo_solve_counted")
     LAUNCHES[0] += 1
 

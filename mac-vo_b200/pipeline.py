@@ -30,6 +30,26 @@ def se3_act(pose: torch.Tensor, p: torch.Tensor) -> torch.Tensor:
     return quat_rotate(pose[3:7].to(p), p) + pose[:3].to(p)
 
 
+def quat_matrix(q: torch.Tensor) -> torch.Tensor:
+    """rotation matrix of q = [x,y,z,w] in q's dtype (pypose `SO3.matrix()`)"""
+    x, y, z, w = q.unbind(-1)
+    return torch.stack([
+        torch.stack([1 - 2 * (y * y + z * z), 2 * (x * y - z * w), 2 * (x * z + y * w)], dim=-1),
+        torch.stack([2 * (x * y + z * w), 1 - 2 * (x * x + z * z), 2 * (y * z - x * w)], dim=-1),
+        torch.stack([2 * (x * z - y * w), 2 * (y * z + x * w), 1 - 2 * (x * x + y * y)], dim=-1),
+    ], dim=-2)
+
+
+class MatchBundle:
+    """the `MatchObs` TensorBundle Odometry/MACVO.py:246-270 hands to the outlier filter: `.data` columns, `len()` rows"""
+
+    def __init__(self, data: dict):
+        self.data = data
+
+    def __len__(self) -> int:
+        return next(iter(self.data.values())).shape[0]
+
+
 @dataclass
 class FrameResult:
     num_kp: int
@@ -47,9 +67,11 @@ class TwoFrameOdometry:
 
     def __init__(self, frontend, kp_selector, cov_model, optimizer, num_point: int = 200, edgewidth: int = 32,
                  match_cov_default: float = 0.25, mapping: bool = True, map_selector=None, min_num_point: int = 10,
-                 keep_debug: bool = False, motion_model=None):
+                 keep_debug: bool = False, motion_model=None, outlier_filter=None):
         self.frontend, self.kp_selector, self.cov_model, self.optimizer = frontend, kp_selector, cov_model, optimizer
         self.motion_model = motion_model            # None: StaticMotionModel (the prediction is the previous pose)
+        self.outlier_filter = outlier_filter        # None: CovarianceSanityFilter
+        self.graph_type = (getattr(optimizer, "context", None) or {}).get("graph_type", "disp")
         self.map_selector = map_selector
         self.num_point, self.edgewidth, self.match_cov_default = num_point, edgewidth, match_cov_default
         self.mapping, self.min_num_point, self.keep_debug = mapping, min_num_point, keep_debug
@@ -62,6 +84,8 @@ class TwoFrameOdometry:
         depth0 = self.frontend.estimate_depth(frame0)
         self.prev = (frame0, depth0)
         self.poses = [torch.tensor([0., 0., 0., 0., 0., 0., 1.])]
+        if self.outlier_filter is not None:
+            self.outlier_filter.set_meta(frame0)
         if self.motion_model is not None:         # the first prediction is the identity (MACVO.initialize)
             self.motion_model.predict(frame0, None, depth0.depth)
 
@@ -111,11 +135,24 @@ class TwoFrameOdometry:
         pos0_cov = self.cov_model.estimate(frame0, kp0_uv, depth0, kp0_sigma_dd, kp0_sigma_uv)
         pos1_cov = self.cov_model.estimate(frame1, kp1_uv, depth1, kp1_sigma_dd, kp1_sigma_uv)
 
-        # CovarianceSanityFilter (Module/OutlierFilter.py:91-100)
-        bad = (pos0_cov.isnan().any(dim=(-1, -2)) | pos0_cov.isinf().any(dim=(-1, -2))
-               | pos1_cov.isnan().any(dim=(-1, -2)) | pos1_cov.isinf().any(dim=(-1, -2)))
-        num_obs = int((~bad).sum())                                    # `bad` lives on the host like the covariances: no sync
-        keep = (~bad).to(dev)
+        kp1_d = None
+        if self.outlier_filter is not None or self.graph_type == "icp":
+            kp1_d = fe.retrieve_pixels(kp1_uv, depth1.depth).squeeze(0)
+        if self.outlier_filter is None:
+            # CovarianceSanityFilter (Module/OutlierFilter.py:91-100)
+            bad = (pos0_cov.isnan().any(dim=(-1, -2)) | pos0_cov.isinf().any(dim=(-1, -2))
+                   | pos1_cov.isnan().any(dim=(-1, -2)) | pos1_cov.isinf().any(dim=(-1, -2)))
+            good = ~bad                                                # lives on the host like the covariances: no sync
+        else:                                                          # Odometry/MACVO.py:246-272
+            placeholder = lambda t: torch.empty((num_kp, 1)).fill_(-1) if t is None else t.unsqueeze(-1).cpu()
+            match_obs = MatchBundle({
+                "pixel1_uv": kp0_uv.cpu(), "pixel2_uv": kp1_uv.cpu(),
+                "pixel1_d": kp0_d.unsqueeze(-1).cpu(), "pixel2_d": kp1_d.unsqueeze(-1).cpu(),
+                "pixel1_d_cov": placeholder(kp0_sigma_dd), "pixel2_d_cov": placeholder(kp1_sigma_dd),
+                "obs1_covTc": pos0_cov, "obs2_covTc": pos1_cov})
+            good = self.outlier_filter.filter(match_obs, torch.device("cpu"))
+        num_obs = int(good.sum())
+        keep = good.to(dev)
         pos_Tw = se3_act(prev_pose.to(dev), pos0_Tc.float())[keep]
 
         self.poses.append(est_pose)
@@ -124,6 +161,11 @@ class TwoFrameOdometry:
             inp = PGOInput(pos_Tw=pos_Tw, kp2_uv=kp1_uv[keep].float(), kp2_disp=kp1_disparity.T[keep],
                            uv_cov=kp1_sigma_uv[keep], disp_cov=kp1_sigma_disparity.T[keep], K=frame1.frame_K,
                            baseline=frame1.frame_baseline, init_pose=est_pose)
+            if self.graph_type == "icp":                               # MACVO.py:274-280, Graphs.py:49-55
+                R = quat_matrix(prev_pose.float()[3:7]).repeat((num_kp, 1, 1)).double()
+                cov_Tw = torch.bmm(torch.bmm(R, pos0_cov), R.transpose(1, 2))
+                good_h = good.cpu()
+                inp.kp2_d, inp.obs_cov, inp.pts_cov = kp1_d[keep], pos1_cov[good_h], cov_Tw[good_h]
             self.optimizer.start_optimize(inp)
             self._pending = True
             out = self.optimizer.get_result() if hasattr(self.optimizer, "optimize_res") else None
@@ -143,7 +185,7 @@ class TwoFrameOdometry:
         if self.keep_debug:
             res.kp0_uv, res.kp1_uv = kp0_uv, kp1_uv
             res.extras = {"depth1": depth1, "match01": match01, "pos0_cov": pos0_cov, "pos1_cov": pos1_cov,
-                          "pos_Tw": pos_Tw, "keep": keep}
+                          "pos_Tw": pos_Tw, "keep": keep, "kp1_d": kp1_d}
         return res
 
     def finish(self) -> torch.Tensor:
@@ -169,14 +211,26 @@ class FusedTwoFrameOdometry:
     `motion_model` (a `plugins.B200_TartanMotionNet`, or None for the previous pose): its graph up to fc1 is enqueued right
     after each frame's frontend, the prefetched next frame's included — it reads only that frame's flow and depth — and
     its head kernel runs in the tail after observe_pack, overwriting the LM's initial pose with the prediction. No extra
-    host synchronisation."""
+    host synchronisation.
+
+    `outlier_filter` (None: CovarianceSanityFilter alone): a B200 observation filter or `B200_FilterCompose` chain that
+    contains `B200_CovarianceSanityFilter`; the whole chain runs inside observe_pack (`plugins.observe_ext`). The graph
+    type comes from `optimizer.context["graph_type"]`; "icp" packs its extra columns into the same buffer and the counted
+    LM reads them there. Either `kp_selector` (B200_CovAwareSelector or its _NoDepth variant) is driven through
+    `enqueue_candidates`."""
 
     def __init__(self, frontend, kp_selector, cov_model, optimizer, num_point: int = 200, edgewidth: int = 32,
                  match_cov_default: float = 0.25, mapping: bool = True, map_selector=None, min_num_point: int = 10,
-                 num_map_point: int = 2000, keep_debug: bool = False, solver=None, motion_model=None):
+                 num_map_point: int = 2000, keep_debug: bool = False, solver=None, motion_model=None,
+                 outlier_filter=None):
         from . import ops
         self.ops = ops
         self.motion_model = motion_model
+        self.outlier_filter = outlier_filter
+        ctx = getattr(optimizer, "context", None) or {}
+        self.graph_type = ctx.get("graph_type", "disp")
+        if solver is not None and self.graph_type != "disp":
+            raise ValueError(f"a custom solver runs the 'disp' graph only (optimizer graph_type {self.graph_type!r})")
         # solver(obs, intr5, pose_io, stats, min_k): the LM solve on the packed observation buffer; default = one persistent
         # launch on this GPU. bench.py --config sharded plugs in the multi-GPU solve (broadcast + sharded_pgo.FusedShardedPGO)
         self.solver = solver
@@ -189,7 +243,9 @@ class FusedTwoFrameOdometry:
         cc = cov_model.config
         self.cov_args = dict(kernel_size=cc.kernel_size, min_flow_cov=cc.min_flow_cov, min_depth_cov=cc.min_depth_cov)
         self.cluster = int(getattr(optimizer, "context", {}).get("cluster", 0)) if hasattr(optimizer, "context") else 0
-        self.obs = [ops.ObservationBuffers(num_point, self.device) for _ in range(2)]      # double buffered
+        icp = self.graph_type == "icp"
+        self.obs = [ops.ObservationBuffers(num_point, self.device, extended=icp) for _ in range(2)]      # double buffered
+        self.ext = None if outlier_filter is None and not icp else {}      # filled by initialize (set_meta resolves "auto")
         self.stats = [torch.zeros((8,), dtype=torch.float64, device=self.device) for _ in range(2)]
         if self.mapping:
             self.map_cov = [torch.empty((num_map_point, 3, 3), dtype=torch.float64, device=self.device) for _ in range(2)]
@@ -210,6 +266,11 @@ class FusedTwoFrameOdometry:
         depth0 = self.frontend.estimate_depth(frame0)
         self.prev = (frame0, depth0)
         self.pose_dev = [torch.tensor([0., 0., 0., 0., 0., 0., 1.], dtype=torch.float64, device=self.device)]
+        if self.ext is not None:
+            from .plugins import observe_ext
+            if self.outlier_filter is not None:
+                self.outlier_filter.set_meta(frame0)
+            self.ext = dict(observe_ext(self.outlier_filter) or {}, icp=self.graph_type == "icp")
 
     @staticmethod
     def _intr(frame) -> tuple[float, float, float, float]:
@@ -236,7 +297,7 @@ class FusedTwoFrameOdometry:
         if self._tail_done is not None:            # the previous frame's tail read the candidate lists the selectors now overwrite
             main.wait_event(self._tail_done)
         # selection kernels for keypoints AND mapping points first, then a single synchronisation for both counts
-        reqs = [(self.kp_selector.enqueue_candidates(match01), self.num_point)]
+        reqs = [(self.kp_selector.enqueue_candidates(frame0, depth0, depth1, match01), self.num_point)]
         if self.mapping:
             reqs.append((self.map_selector.enqueue_candidates(depth0), self.num_map_point))
         counts = ops.request_candidate_counts(reqs)
@@ -250,7 +311,8 @@ class FusedTwoFrameOdometry:
             self._tail_stream = torch.cuda.Stream(self.device)
         tail = self._tail_stream
         tail.wait_event(counts)
-        for t in (match01.flow, match01.cov, depth0.depth, depth1.depth, depth1.disparity, depth1.disparity_uncertainty, fc1):
+        for t in (match01.flow, match01.cov, depth0.depth, depth1.depth, depth1.disparity, depth1.disparity_uncertainty, fc1,
+                  depth0.cov, depth1.cov):
             if t is not None:
                 t.record_stream(tail)          # allocated on the main stream, consumed on the tail stream
         with torch.cuda.stream(tail):
@@ -274,9 +336,10 @@ class FusedTwoFrameOdometry:
         obs, stats = self.obs[slot], self.stats[slot]
         next_pose = torch.empty((7,), dtype=torch.float64, device=self.device)
         i0, i1 = self._intr(frame0), self._intr(frame1)
+        ext = None if self.ext is None else dict(self.ext, depth_cov0=depth0.cov, depth_cov1=depth1.cov)
         ops.observe_pack(obs, kp0_uv, match01.flow, match01.cov, depth0.depth, depth1.depth, depth1.disparity,
                          depth1.disparity_uncertainty, self.edgewidth, i0, i1, self.pose_dev[-1], next_pose,
-                         match_cov_default=self.match_cov_default, **self.cov_args)
+                         match_cov_default=self.match_cov_default, ext=ext, **self.cov_args)
         if fc1 is not None:     # the motion model's prediction replaces observe_pack's previous-pose prior
             self.motion_model.head(fc1, self.pose_dev[-1], next_pose)
         pose_init = next_pose.clone() if self.keep_debug else None      # the LM's initial pose, before the solve
@@ -285,7 +348,8 @@ class FusedTwoFrameOdometry:
         if self.solver is not None:
             self.solver(obs, (*i1, bl), next_pose, stats, self.min_num_point)
         else:
-            ops.pgo_solve_counted(obs, (*i1, bl), next_pose, stats, min_k=self.min_num_point, cluster=self.cluster)
+            ops.pgo_solve_counted(obs, (*i1, bl), next_pose, stats, min_k=self.min_num_point, cluster=self.cluster,
+                                  graph_type=self.graph_type)
         self.pose_dev.append(next_pose)
         n_map = 0
         if self.mapping:
@@ -327,9 +391,11 @@ class FusedTwoFrameOdometry:
         obs.ready.synchronize()
         hdr = obs.section("header", host=True)
         n = int(hdr[0])
-        out = {k: obs.section(k, host=True)[:n].clone() for k in
-               ("pos_Tw", "pixel2_uv", "pixel2_disp", "pixel2_uv_cov", "pixel2_disp_cov", "obs1_covTc", "obs2_covTc",
-                "pixel1_uv", "pixel1_d")}
+        names = ("pos_Tw", "pixel2_uv", "pixel2_disp", "pixel2_uv_cov", "pixel2_disp_cov", "obs1_covTc", "obs2_covTc",
+                 "pixel1_uv", "pixel1_d")
+        if obs.extended:
+            names += ("pixel2_d", "pixel1_d_cov", "pixel2_d_cov", "points_Tc", "cov_Tw")
+        out = {k: obs.section(k, host=True)[:n].clone() for k in names}
         out.update(num_obs=n, num_kp=int(hdr[1]), num_selected=int(hdr[2]), status=int(hdr[3]))
         if self.mapping:
             self.pose_ready[slot].synchronize()

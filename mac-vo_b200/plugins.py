@@ -6,6 +6,9 @@
     B200_MappingPointSelector        IKeypointSelector  replaces MappingPointSelector (KeypointSelector.py:78-100)
     B200_MatchCovariance             ICovariance2to3    replaces MatchCovariance (Covariance/Project2to3.py:114-182)
     B200_CovarianceSanityFilter      IObservationFilter replaces CovarianceSanityFilter (OutlierFilter.py:91-100)
+    B200_SimpleDepthFilter           IObservationFilter replaces SimpleDepthFilter (OutlierFilter.py:103-124)
+    B200_LikelyFrontOfCamFilter      IObservationFilter replaces LikelyFrontOfCamFilter (OutlierFilter.py:127-141)
+    B200_FilterCompose               IObservationFilter replaces FilterCompose (OutlierFilter.py:44-75)
     B200_MotionInterpolate           IMapProcessor      replaces MotionInterpolate (MapProcessor.py:52-79)
     B200_TwoFrame_PGO                IOptimizer         replaces TwoFrame_PGO (Optimization/TwoFramePGO/Optimizer.py:23-108)
     B200_TartanMotionNet             IMotionModel       replaces TartanMotionNet (MotionModel.py:89-116)
@@ -239,8 +242,9 @@ class B200_CovAwareSelector_NoDepth(IKeypointSelector):
         self._cand: ops.CandidateList | None = None
 
     @torch.inference_mode()
-    def enqueue_candidates(self, match_est) -> "ops.CandidateList":
-        """Kernels only (median threshold, flags, ordered compaction) — no host synchronisation."""
+    def enqueue_candidates(self, frame, depth0_est, depth1_est, match_est) -> "ops.CandidateList":
+        """Kernels only (median threshold, flags, ordered compaction) — no host synchronisation. Takes `select_point`'s
+        arguments (the depth estimates are not read) so that callers drive either CovAware selector the same way."""
         if match_est is None or match_est.cov is None:
             raise ValueError("B200_CovAwareSelector_NoDepth needs match_est.cov (the reference falls back to a grid "
                              "selector here; compose it with GridSelector in the YAML if that is wanted)")
@@ -265,7 +269,7 @@ class B200_CovAwareSelector_NoDepth(IKeypointSelector):
 
     @torch.inference_mode()
     def select_point(self, frame, numPoint: int, depth0_est, depth1_est, match_est) -> torch.Tensor:
-        return ops.sample_candidates(self.enqueue_candidates(match_est), numPoint)
+        return ops.sample_candidates(self.enqueue_candidates(frame, depth0_est, depth1_est, match_est), numPoint)
 
     @classmethod
     def is_valid_config(cls, config: SimpleNamespace | None) -> None:
@@ -288,7 +292,8 @@ class B200_CovAwareSelector(IKeypointSelector):
         self._cand: ops.CandidateList | None = None
 
     @torch.inference_mode()
-    def select_point(self, frame, numPoint: int, depth0_est, depth1_est, match_est) -> torch.Tensor:
+    def enqueue_candidates(self, frame, depth0_est, depth1_est, match_est) -> "ops.CandidateList":
+        """Kernels only (scores, median thresholds, flags, ordered compaction) — no host synchronisation."""
         assert depth0_est.cov is not None
         assert depth1_est.cov is not None
         if match_est is None or match_est.cov is None:
@@ -304,7 +309,11 @@ class B200_CovAwareSelector(IKeypointSelector):
         ops.select_candidates_depth(self._score, depth0_est.depth.to(dev), depth1_est.depth.to(dev), depth0_est.cov.to(dev),
                                     self.config.mask_width, self.config.max_depth, self.config.max_depth_cov,
                                     self.config.max_match_cov, depth0_est.mask, match_est.mask, self._cand)
-        return ops.sample_candidates(self._cand, numPoint)
+        return self._cand
+
+    @torch.inference_mode()
+    def select_point(self, frame, numPoint: int, depth0_est, depth1_est, match_est) -> torch.Tensor:
+        return ops.sample_candidates(self.enqueue_candidates(frame, depth0_est, depth1_est, match_est), numPoint)
 
     @classmethod
     def is_valid_config(cls, config: SimpleNamespace | None) -> None:
@@ -433,6 +442,126 @@ class B200_CovarianceSanityFilter(IObservationFilter):
     @classmethod
     def is_valid_config(cls, config: SimpleNamespace | None) -> None:
         return
+
+    def observe_ext(self) -> dict:
+        """what `macvo_observe_pack` needs to run this filter: nothing, observe_kernel always applies it"""
+        return {}
+
+
+def _column(values, key: str) -> torch.Tensor:
+    t = values.data[key]
+    return t.tensor if hasattr(t, "tensor") and not isinstance(t, torch.Tensor) else t
+
+
+class B200_SimpleDepthFilter(IObservationFilter):
+    """Replacement of SimpleDepthFilter (Module/OutlierFilter.py:103-124): drops observations whose depth lies below
+    min_depth or above max_depth on either frame (a NaN depth passes). `max_depth: auto` becomes fx * baseline in
+    `set_meta`. On the device the test runs inside observe_kernel (`observe_ext`)."""
+
+    def set_meta(self, meta) -> None:
+        if self.config.max_depth == "auto":
+            self.config.max_depth = meta.fx * meta.frame_baseline
+
+    @property
+    def required_keys(self) -> set:
+        return {"pixel1_d", "pixel2_d"}
+
+    def filter(self, values, device: torch.device) -> torch.Tensor:
+        d1, d2 = _column(values, "pixel1_d"), _column(values, "pixel2_d")
+        lo, hi = self.config.min_depth, self.config.max_depth
+        return (~((d1 < lo) | (d1 > hi) | (d2 < lo) | (d2 > hi)).squeeze(-1)).to(device)
+
+    def observe_ext(self) -> dict:
+        if self.config.max_depth == "auto":
+            raise ValueError("B200_SimpleDepthFilter: max_depth 'auto' is resolved by set_meta(); call it first")
+        # the reference compares fp32 tensors with python floats: the thresholds act rounded to fp32
+        return {"simple_depth": True, "min_depth": float(self.config.min_depth), "max_depth": float(self.config.max_depth)}
+
+    @classmethod
+    def is_valid_config(cls, config: SimpleNamespace | None) -> None:
+        assert config is not None
+        if isinstance(config.max_depth, (float, int)):
+            assert config.max_depth > config.min_depth
+        cls._enforce_config_spec(config, {
+            "min_depth": lambda dist: isinstance(dist, (int, float)) and dist > 0.,
+            "max_depth": lambda dist: (dist == "auto") or (isinstance(dist, (int, float)) and dist > 0.),
+        })
+
+
+class B200_LikelyFrontOfCamFilter(IObservationFilter):
+    """Replacement of LikelyFrontOfCamFilter (Module/OutlierFilter.py:127-141): keeps observations with
+    d - 2 sqrt(d_cov) > 0 on both frames; passes everything when any pixel1_d_cov is the -1 placeholder of a frontend
+    without depth covariance. On the device: observe_kernel / pack_kernel (`observe_ext`)."""
+
+    @property
+    def required_keys(self) -> set:
+        return {"pixel1_d", "pixel1_d_cov", "pixel2_d", "pixel2_d_cov"}
+
+    def filter(self, values, device: torch.device) -> torch.Tensor:
+        d1, c1 = _column(values, "pixel1_d"), _column(values, "pixel1_d_cov")
+        d2, c2 = _column(values, "pixel2_d"), _column(values, "pixel2_d_cov")
+        if (c1 == -1).any():
+            return torch.ones((d1.shape[0],), dtype=torch.bool, device=device)
+        return (((d1 - (c1.sqrt() * 2)) > 0.) & ((d2 - (c2.sqrt() * 2)) > 0.)).squeeze(-1).to(device)
+
+    def observe_ext(self) -> dict:
+        return {"front_of_cam": True}
+
+    @classmethod
+    def is_valid_config(cls, config: SimpleNamespace | None) -> None:
+        return
+
+
+class B200_FilterCompose(IObservationFilter):
+    """Replacement of FilterCompose (Module/OutlierFilter.py:44-75): the AND of its filters' masks. `filter_args` may
+    name B200 filters only. The fused driver runs the whole chain inside `macvo_observe_pack` (`observe_ext`)."""
+
+    def __init__(self, config: SimpleNamespace):
+        super().__init__(config)
+        self.filters = [IObservationFilter.instantiate(a.type, a.args) for a in self.config.filter_args]
+
+    @property
+    def required_keys(self) -> set:
+        return {k for f in self.filters for k in f.required_keys}
+
+    def set_meta(self, meta) -> None:
+        for f in self.filters:
+            f.set_meta(meta)
+
+    def filter(self, values, device: torch.device) -> torch.Tensor:
+        mask = torch.ones((len(values),), dtype=torch.bool, device=device)
+        for f in self.filters:
+            mask = torch.logical_and(mask, f.filter(values, device))
+        return mask
+
+    def observe_ext(self) -> dict:
+        ext: dict = {}
+        for f in self.filters:
+            if not hasattr(f, "observe_ext"):
+                raise ValueError(f"B200_FilterCompose: {type(f).__name__} has no device implementation")
+            ext.update(f.observe_ext())
+        return ext
+
+    @classmethod
+    def is_valid_config(cls, config: SimpleNamespace | None) -> None:
+        assert config is not None
+        assert isinstance(config.filter_args, list)
+        for filter_arg in config.filter_args:
+            IObservationFilter.is_valid_config(filter_arg)
+
+
+def observe_ext(outlier_filter) -> dict | None:
+    """`macvo_observe_pack`'s extension for an outlier filter (None: CovarianceSanityFilter alone, which observe_kernel
+    always applies). Raises for a filter the device path cannot run, or a chain without the sanity filter."""
+    if outlier_filter is None:
+        return None
+    chain = outlier_filter.filters if isinstance(outlier_filter, B200_FilterCompose) else [outlier_filter]
+    if not any(isinstance(f, B200_CovarianceSanityFilter) for f in chain):
+        raise ValueError("the device observation path always applies CovarianceSanityFilter: the outlier filter must "
+                         "contain B200_CovarianceSanityFilter")
+    if not hasattr(outlier_filter, "observe_ext"):
+        raise ValueError(f"{type(outlier_filter).__name__} has no device implementation")
+    return outlier_filter.observe_ext()
 
 
 # ================================================================================================
