@@ -401,6 +401,7 @@ int macvo_convex_upsample(const float* flow, const float* mask_nhwc, float* out,
  * *status (zeroed by the caller) is a bitmask, OR-ed by every observation that meets a condition:
  *   bit 0 (1): a covariance patch crossed the bottom or right image edge (the reference raises IndexError; those
  *              rows' covariances are unspecified). Patches crossing the top / left edge wrap like python indices.
+ *              Never set with the NoCovariance model (ext->cov_model == MACVO_COV_IDENTITY), which reads no patch.
  *   bit 1 (2): a keypoint kp0 lies outside the image; its row is dropped and not counted in n_inbound.
  */
 /* CovarianceSanityFilter.filter (Module/OutlierFilter.py:91-100) on device-resident (k,3,3) float64 covariances:
@@ -418,7 +419,20 @@ int macvo_cov_sanity_filter(const double* obs1_cov, const double* obs2_cov, int 
  *                 fp32, computed in fp32, widened) for the kept rows, AFTER the header (every offset above stays):
  *   [31c+4,32c+4) pixel2_d | [32c+4,33c+4) pixel1_d_cov | [33c+4,34c+4) pixel2_d_cov | [34c+4,37c+4) points_Tc (c,3)
  *   [37c+4,46c+4) cov_Tw (c,3,3)        -> `packed` must hold macvo_observe_packed_doubles(capacity, 1) = 46c + 4 doubles.
- * macvo_observe_packed_doubles(capacity, 0) = 31c + 4. */
+ * macvo_observe_packed_doubles(capacity, 0) = 31c + 4.
+ *
+ * The covariance model of the ablation configs (Module/Covariance/Project2to3.py:48-57, 281-323); all zero = MatchCovariance
+ * without modifiers, exactly the behaviour above:
+ *   cov_model     MACVO_COV_MATCH, or MACVO_COV_IDENTITY (NoCovariance: no depth taps, the uv-covariance columns hold the
+ *                 network's values unclamped, status bit 0 is never set, both 3x3 covariances are the identity);
+ *   cov_ops[0..n_cov_ops)  modifiers in the order they apply (innermost wrapper first), in float64 on the widened fp32
+ *                 covariances, BEFORE the sanity filter, the obs1_covTc / obs2_covTc columns and cov_Tw (see macvo_cov_modify).
+ * Setting only these fields (no filter, icp 0) keeps the 31c + 4 layout and applies the sanity filter alone. */
+#define MACVO_COV_MATCH 0
+#define MACVO_COV_IDENTITY 1
+#define MACVO_COV_DIAGONALIZE 1
+#define MACVO_COV_NORMALIZE 2
+#define MACVO_COV_MAX_OPS 2
 typedef struct {
     const float* depth_cov0; /* (h,w) device, or NULL */
     const float* depth_cov1; /* (h,w) device, or NULL */
@@ -426,7 +440,17 @@ typedef struct {
     float min_depth, max_depth;
     int front_of_cam;
     int icp;
+    int cov_model;
+    int cov_ops[MACVO_COV_MAX_OPS];
+    int n_cov_ops;
 } macvo_observe_ext_t;
+/* The covariance modifiers on device (k,3,3) float64 matrices, in place, applied in the order of the HOST array ops[0..n_ops):
+ *   MACVO_COV_DIAGONALIZE  Modifier_Diagonalize: the six off-diagonal entries become 0 (a NaN / Inf there disappears);
+ *   MACVO_COV_NORMALIZE    Modifier_Normalize: each matrix divided by ITS OWN determinant, from a 3x3 LU with partial
+ *                          pivoting (largest |a|, first on ties; multipliers by division; det = sign u00 u11 u22), each
+ *                          element divided (round-to-nearest) — det 0 gives +-Inf / NaN, a negative det flips the sign.
+ * n_ops <= MACVO_COV_MAX_OPS. The same routine runs inside macvo_observe_pack. */
+int macvo_cov_modify(double* cov, int k, const int* ops, int n_ops, void* stream);
 size_t macvo_observe_workspace_bytes(int capacity);
 size_t macvo_observe_packed_doubles(int capacity, int extended);
 int macvo_observe_pack(const int64_t* kp0_uv, int k, int capacity, const float* flow, const float* match_cov,

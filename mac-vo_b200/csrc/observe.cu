@@ -13,6 +13,9 @@
 //                    all inside ONE buffer so that a single asynchronous device->host copy ships a frame's
 //                    observations; the survivor count stays on the device (pgo_lm_kernel reads it there).
 //
+// With a macvo_observe_ext_t the covariance model of the ablation configs replaces MatchCovariance: NoCovariance (identity,
+// no depth taps) and the Diagonalize / Normalize modifiers (cov_modify9, shared with macvo_cov_modify).
+//
 // Arithmetic: fp32 in the reference's operation order (explicit round-to-nearest intrinsics, no contraction), widened
 // to fp64 exactly where the reference calls `.double()`.
 #include "cov2to3.cuh"
@@ -39,6 +42,9 @@ struct ObserveArgs {
     const float* depth_cov0;       // (h,w) or nullptr (-1 placeholder)
     const float* depth_cov1;
     float* rex;                    // (k, REX) extension records
+    int identity;                  // NoCovariance: no depth taps, raw uv covariances, identity 3x3 covariances
+    int n_ops, op0, op1;           // covariance modifiers, op0 first
+    double* rcov;                  // (k, RCOV) modified covariances (n_ops > 0 only)
 };
 
 // record slot (floats): 0 keep | 1,2 kp1 uv | 3 depth0 | 4 disp1 | 5 disp_unc1 | 6..8 uv cov (clamped) | 9..11 pos_Tw |
@@ -46,12 +52,81 @@ struct ObserveArgs {
 constexpr int REC = 25;
 // extension record (ext only): 0 pixel2_d | 1 pixel1_d_cov | 2 pixel2_d_cov | 3 LikelyFrontOfCam verdict | 4..6 points_Tc
 constexpr int REX = 7;
+// modified-covariance record (float64, only with modifiers): 0..8 cov0 (3,3) | 9..17 cov1 (3,3).
+// A modified covariance is float64 and no longer fits the fp32 record. observe_kernel, which needs it for the keep decision
+// anyway, stores it here and pack_kernel copies it: recomputing the LU in pack_kernel (1024 threads, so at most 64
+// registers) spills, and the keep decision and the packed values are then the same numbers by construction.
+constexpr int RCOV = 18;
+static_assert((REC + REX) % 2 == 0, "the float64 records after the fp32 ones must stay 8-byte aligned");
 
 __device__ __forceinline__ bool bad6(const float* s) {
     bool b = false;
 #pragma unroll
     for (int i = 0; i < 6; ++i) b |= !isfinite(s[i]);
     return b;
+}
+
+__device__ __forceinline__ bool bad9(const double* m) {
+    bool b = false;
+#pragma unroll
+    for (int i = 0; i < 9; ++i) b |= !isfinite(m[i]);
+    return b;
+}
+
+// torch.det of a 3x3 float64 matrix as an LU factorisation with partial pivoting: pivot = largest |a| of the column (the
+// first on ties; a NaN is never preferred), multipliers by division (a zero pivot leaves its column unscaled, like LAPACK's
+// getrf, and the trailing update still runs); det = sign * u00 * u11 * u22 (the product of the diagonal, then the sign)
+// CPU torch.det hands the row-major matrix to column-major LAPACK, so it factors the TRANSPOSE (det A^T = det A); so does
+// this routine, which makes the NaN / Inf / signed-zero class of the result agree with it, not only its value
+__device__ __forceinline__ double det3_lu(const double* m) {
+    double a[9];
+#pragma unroll
+    for (int e = 0; e < 9; ++e) a[e] = m[3 * (e % 3) + e / 3];
+    double sign = 1.0;
+#pragma unroll
+    for (int j = 0; j < 2; ++j) {
+        int p = j;
+        double best = fabs(a[3 * j + j]);
+#pragma unroll
+        for (int i = j + 1; i < 3; ++i)
+            if (fabs(a[3 * i + j]) > best) { best = fabs(a[3 * i + j]); p = i; }
+        if (p != j) sign = -sign;
+#pragma unroll
+        for (int i = j + 1; i < 3; ++i)             // row swap with constant indices only: the matrix stays in registers
+            if (p == i) {
+#pragma unroll
+                for (int c = j; c < 3; ++c) { const double t = a[3 * j + c]; a[3 * j + c] = a[3 * i + c]; a[3 * i + c] = t; }
+            }
+        const double piv = a[3 * j + j];
+#pragma unroll
+        for (int i = j + 1; i < 3; ++i) {
+            const double l = piv != 0.0 ? __ddiv_rn(a[3 * i + j], piv) : a[3 * i + j];
+#pragma unroll
+            for (int c = j + 1; c < 3; ++c) a[3 * i + c] = __dsub_rn(a[3 * i + c], __dmul_rn(l, a[3 * j + c]));
+        }
+    }
+    return __dmul_rn(__dmul_rn(__dmul_rn(a[0], a[4]), a[8]), sign);
+}
+
+// The covariance modifiers (Project2to3.py:281-323) on one (3,3) float64 matrix, ops[0] first (the innermost wrapper).
+// observe_kernel (keep decision), pack_kernel (the packed columns, cov_Tw) and macvo_cov_modify all call this one routine.
+__device__ __forceinline__ void cov_modify9(double* m, int n_ops, int op0, int op1) {
+    for (int o = 0; o < n_ops; ++o) {
+        const int op = o == 0 ? op0 : op1;
+        if (op == MACVO_COV_DIAGONALIZE) {
+            m[1] = m[2] = m[3] = m[5] = m[6] = m[7] = 0.0;
+        } else {                                                     // MACVO_COV_NORMALIZE: covs /= det(covs)
+            const double det = det3_lu(m);
+#pragma unroll
+            for (int e = 0; e < 9; ++e) m[e] = __ddiv_rn(m[e], det);
+        }
+    }
+}
+
+// the base model's six fp32 entries, widened, then the modifiers
+__device__ __forceinline__ void modified_cov9(double* m, const float* s6, int n_ops, int op0, int op1) {
+    macvo::store_cov9(m, s6);
+    cov_modify9(m, n_ops, op0, op1);
 }
 
 __global__ void __launch_bounds__(128)
@@ -84,20 +159,44 @@ observe_kernel(ObserveArgs A, float* __restrict__ rec, int* __restrict__ status)
     const int p1 = (int)(vl1 * A.w + ul1);                            // inside the image: edge > 0
     const float d0 = A.depth0[p0];
     const float disp1 = A.disparity1[p1], dunc1 = A.disp_unc1[p1];
-    // frame-0 keypoints: constant quantisation covariance, clamped like any flow_cov (Project2to3.py:130-133)
-    const float s0 = fmaxf(A.match_cov_default, A.min_flow_var);
     float c0[6], c1[6];
-    bool oob = macvo::match_cov_warp((float)u0, (float)v0, u0, v0, A.depth0, A.h, A.w, s0, s0, 0.f, false, 0.f, A.P0, lane, c0);
-    // frame-1 keypoints: the network's match covariance at the source pixel, clamped in place
     const float a = A.match_cov[p0], b = A.match_cov[hw + p0];
-    const float suu = (a != a) ? a : fmaxf(a, A.min_flow_var);
-    const float svv = (b != b) ? b : fmaxf(b, A.min_flow_var);
     const float suv = A.match_cov[2 * hw + p0];
-    oob |= macvo::match_cov_warp(u1, v1, ul1, vl1, A.depth1, A.h, A.w, suu, svv, suv, false, 0.f, A.P1, lane, c1);
-    if (lane != 0) return;
+    float suu, svv;
+    bool oob = false;
+    if (A.identity) {
+        // NoCovariance.estimate (Project2to3.py:52-54): identity, no patch read, flow_cov left as the network gave it
+        if (lane != 0) return;
+        suu = a; svv = b;
+#pragma unroll
+        for (int e = 0; e < 6; ++e) c0[e] = c1[e] = (e == 0 || e == 3 || e == 5) ? 1.f : 0.f;
+    } else {
+        // frame-0 keypoints: constant quantisation covariance, clamped like any flow_cov (Project2to3.py:130-133)
+        const float s0 = fmaxf(A.match_cov_default, A.min_flow_var);
+        oob = macvo::match_cov_warp((float)u0, (float)v0, u0, v0, A.depth0, A.h, A.w, s0, s0, 0.f, false, 0.f, A.P0, lane, c0);
+        // frame-1 keypoints: the network's match covariance at the source pixel, clamped in place
+        suu = (a != a) ? a : fmaxf(a, A.min_flow_var);
+        svv = (b != b) ? b : fmaxf(b, A.min_flow_var);
+        oob |= macvo::match_cov_warp(u1, v1, ul1, vl1, A.depth1, A.h, A.w, suu, svv, suv, false, 0.f, A.P1, lane, c1);
+        if (lane != 0) return;
+    }
     if (oob) atomicOr(status, 1);                // status is a bitmask: both conditions may occur in one call
-    // CovarianceSanityFilter: drop observations with NaN / Inf covariance on either frame
-    bool keep = !(bad6(c0) || bad6(c1));
+    // CovarianceSanityFilter: drop observations with NaN / Inf covariance on either frame, after the modifiers
+    bool keep;
+    if (A.n_ops == 0) {
+        keep = !(bad6(c0) || bad6(c1));
+    } else {
+        double m[9];
+        double* w = A.rcov + (long long)i * RCOV;
+        modified_cov9(m, c0, A.n_ops, A.op0, A.op1);
+        keep = !bad9(m);
+#pragma unroll
+        for (int e = 0; e < 9; ++e) w[e] = m[e];
+        modified_cov9(m, c1, A.n_ops, A.op0, A.op1);
+        keep &= !bad9(m);
+#pragma unroll
+        for (int e = 0; e < 9; ++e) w[9 + e] = m[e];
+    }
     if (A.ext) {
         // Module/OutlierFilter.py:106-141 in fp32 on the MatchObs columns (MACVO.py:205-248 gathers)
         const float d1 = A.depth1[p1];
@@ -144,6 +243,7 @@ struct PackExt {
     int on, front_of_cam, icp;
     const float* rex;
     const double* prev_pose;
+    const double* rcov;            // observe_kernel's modified covariances, or nullptr (no modifier)
 };
 
 // packed float64 buffer, sections sized by the CAPACITY cap (fixed pointers for the LM kernel):
@@ -207,8 +307,14 @@ pack_kernel(const float* __restrict__ rec, const int64_t* __restrict__ kp0, int 
             out[5 * c + j] = r[4];
             out[6 * c + 3 * j] = r[6]; out[6 * c + 3 * j + 1] = r[7]; out[6 * c + 3 * j + 2] = r[8];
             out[9 * c + j] = r[5];
-            macvo::store_cov9(out + 10 * c + 9LL * j, r + 12);
-            macvo::store_cov9(out + 19 * c + 9LL * j, r + 18);
+            if (!X.rcov) {
+                macvo::store_cov9(out + 10 * c + 9LL * j, r + 12);
+                macvo::store_cov9(out + 19 * c + 9LL * j, r + 18);
+            } else {
+                const double* m = X.rcov + (long long)i * RCOV;
+#pragma unroll
+                for (int e = 0; e < 9; ++e) { out[10 * c + 9LL * j + e] = m[e]; out[19 * c + 9LL * j + e] = m[9 + e]; }
+            }
             out[28 * c + 2 * j] = (double)kp0[2 * i]; out[28 * c + 2 * j + 1] = (double)kp0[2 * i + 1];
             out[30 * c + j] = r[3];
             if (X.icp) {
@@ -216,8 +322,13 @@ pack_kernel(const float* __restrict__ rec, const int64_t* __restrict__ kp0, int 
                 e[j] = x[0]; e[c + j] = x[1]; e[2 * c + j] = x[2];
                 e[3 * c + 3 * j] = x[4]; e[3 * c + 3 * j + 1] = x[5]; e[3 * c + 3 * j + 2] = x[6];
                 // cov_Tw = R obs1_covTc R^T in float64 (torch.bmm(torch.bmm(R, cov), R^T), MACVO.py:280)
-                double C[9], RC[9];
-                macvo::store_cov9(C, r + 12);
+                double C[9], RC[9];                                 // obs1_covTc as packed above (modifiers applied)
+                if (!X.rcov) {
+                    macvo::store_cov9(C, r + 12);
+                } else {
+#pragma unroll
+                    for (int e = 0; e < 9; ++e) C[e] = X.rcov[(long long)i * RCOV + e];
+                }
 #pragma unroll
                 for (int a = 0; a < 3; ++a)
 #pragma unroll
@@ -252,7 +363,35 @@ __global__ void cov_sanity_kernel(const double* __restrict__ c1, const double* _
     good[i] = ok ? 1 : 0;
 }
 
+// macvo_cov_modify: one thread per (3,3) matrix, in place
+__global__ void cov_modify_kernel(double* __restrict__ cov, int k, int n_ops, int op0, int op1) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= k) return;
+    double m[9];
+#pragma unroll
+    for (int e = 0; e < 9; ++e) m[e] = cov[9LL * i + e];
+    cov_modify9(m, n_ops, op0, op1);
+#pragma unroll
+    for (int e = 0; e < 9; ++e) cov[9LL * i + e] = m[e];
+}
+
+bool valid_cov_ops(const int* ops, int n_ops) {
+    if (n_ops < 0 || n_ops > MACVO_COV_MAX_OPS || (n_ops > 0 && !ops)) return false;
+    for (int o = 0; o < n_ops; ++o)
+        if (ops[o] != MACVO_COV_DIAGONALIZE && ops[o] != MACVO_COV_NORMALIZE) return false;
+    return true;
+}
+
 }  // namespace
+
+extern "C" int macvo_cov_modify(double* cov, int k, const int* ops, int n_ops, void* stream) {
+    if (k < 0 || !valid_cov_ops(ops, n_ops)) return MACVO_E_ARG;
+    if (k == 0 || n_ops == 0) return MACVO_OK;
+    if (!cov) return MACVO_E_ARG;
+    cov_modify_kernel<<<ceil_div(k, 256), 256, 0, as_stream(stream)>>>(cov, k, n_ops, ops[0], n_ops > 1 ? ops[1] : 0);
+    MACVO_LAUNCH_CHECK();
+    return MACVO_OK;
+}
 
 extern "C" int macvo_cov_sanity_filter(const double* obs1_cov, const double* obs2_cov, int k, uint8_t* good, void* stream) {
     if (k < 0) return MACVO_E_ARG;
@@ -264,7 +403,8 @@ extern "C" int macvo_cov_sanity_filter(const double* obs1_cov, const double* obs
 }
 
 extern "C" size_t macvo_observe_workspace_bytes(int capacity) {
-    return (size_t)capacity * (REC + REX) * sizeof(float);
+    // the fp32 records, then the float64 modified covariances
+    return (size_t)capacity * ((REC + REX) * sizeof(float) + RCOV * sizeof(double));
 }
 
 extern "C" size_t macvo_observe_packed_doubles(int capacity, int extended) {
@@ -286,6 +426,9 @@ extern "C" int macvo_observe_pack(const int64_t* kp0_uv, int k, int capacity, co
         return MACVO_E_ARG;
     if (workspace_bytes < macvo_observe_workspace_bytes(capacity)) return MACVO_E_WORKSPACE;
     if (ext && ext->simple_depth && !(ext->min_depth <= ext->max_depth)) return MACVO_E_ARG;
+    if (ext && ((ext->cov_model != MACVO_COV_MATCH && ext->cov_model != MACVO_COV_IDENTITY) ||
+                !valid_cov_ops(ext->cov_ops, ext->n_cov_ops)))
+        return MACVO_E_ARG;
     ObserveArgs A;
     A.kp0 = kp0_uv; A.k = k; A.flow = flow; A.match_cov = match_cov; A.depth0 = depth0; A.depth1 = depth1;
     A.disparity1 = disparity1; A.disp_unc1 = disp_unc1; A.h = h; A.w = w; A.edge = edge_width;
@@ -300,7 +443,12 @@ extern "C" int macvo_observe_pack(const int64_t* kp0_uv, int k, int capacity, co
     A.min_depth = ext ? ext->min_depth : 0.f; A.max_depth = ext ? ext->max_depth : 0.f;
     A.depth_cov0 = ext ? ext->depth_cov0 : nullptr; A.depth_cov1 = ext ? ext->depth_cov1 : nullptr;
     A.rex = rec + (size_t)capacity * REC;
-    PackExt X{A.ext, A.front_of_cam, ext && ext->icp, A.rex, prev_pose};
+    A.identity = ext && ext->cov_model == MACVO_COV_IDENTITY;
+    A.n_ops = ext ? ext->n_cov_ops : 0;
+    A.op0 = A.n_ops > 0 ? ext->cov_ops[0] : 0;
+    A.op1 = A.n_ops > 1 ? ext->cov_ops[1] : 0;
+    A.rcov = reinterpret_cast<double*>(A.rex + (size_t)capacity * REX);
+    PackExt X{A.ext, A.front_of_cam, ext && ext->icp, A.rex, prev_pose, A.n_ops > 0 ? A.rcov : nullptr};
     cudaStream_t st = as_stream(stream);
     observe_kernel<<<max(1, ceil_div(k * 32, 128)), 128, 0, st>>>(A, rec, status);
     MACVO_LAUNCH_CHECK();

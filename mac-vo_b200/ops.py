@@ -39,7 +39,8 @@ class _ScoreT(C.Structure):
 
 class _ObserveExt(C.Structure):
     _fields_ = [("depth_cov0", C.c_void_p), ("depth_cov1", C.c_void_p), ("simple_depth", C.c_int),
-                ("min_depth", C.c_float), ("max_depth", C.c_float), ("front_of_cam", C.c_int), ("icp", C.c_int)]
+                ("min_depth", C.c_float), ("max_depth", C.c_float), ("front_of_cam", C.c_int), ("icp", C.c_int),
+                ("cov_model", C.c_int), ("cov_ops", C.c_int * 2), ("n_cov_ops", C.c_int)]
 
 
 class _PgoParams(C.Structure):
@@ -77,6 +78,7 @@ EXPORTS = {
     "macvo_motion_interpolate_workspace_bytes": (C.c_size_t, [C.c_int]),
     "macvo_motion_interpolate": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     "macvo_cov_sanity_filter": (C.c_int, [C.c_void_p] * 2 + [C.c_int] + [C.c_void_p] * 2),
+    "macvo_cov_modify": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p]),
     "macvo_observe_workspace_bytes": (C.c_size_t, [C.c_int]),
     "macvo_observe_packed_doubles": (C.c_size_t, [C.c_int, C.c_int]),
     "macvo_observe_pack": (C.c_int, [C.c_void_p, C.c_int, C.c_int] + [C.c_void_p] * 6 + [C.c_int] * 3 + [C.c_void_p] * 2
@@ -653,6 +655,32 @@ def cov_sanity_filter(obs1_cov: Tensor, obs2_cov: Tensor) -> Tensor:
     return good.bool()
 
 
+COV_MODELS = {"match": 0, "identity": 1}              # macvo_observe_ext_t.cov_model (MACVO_COV_MATCH / _IDENTITY)
+COV_OPS = {"diagonalize": 1, "normalize": 2}          # MACVO_COV_DIAGONALIZE / MACVO_COV_NORMALIZE
+
+
+def _cov_ops(ops: list[str] | tuple[str, ...], what: str):
+    bad = [o for o in ops if o not in COV_OPS]
+    if bad or len(ops) > 2:
+        raise MacvoB200Error(f"{what}: covariance modifiers must be at most two of {sorted(COV_OPS)}, got {list(ops)}")
+    return (C.c_int * 2)(*([COV_OPS[o] for o in ops] + [0] * (2 - len(ops))))
+
+
+def cov_modify(cov: Tensor, ops: list[str] | tuple[str, ...]) -> Tensor:
+    """Modifier_Diagonalize / Modifier_Normalize (Project2to3.py:281-323) in place on a contiguous (K,3,3) float64 CUDA
+    tensor; `ops` in the order they apply (the innermost wrapper first). Returns `cov`."""
+    arr = _cov_ops(ops, "cov_modify")
+    if not (isinstance(cov, Tensor) and cov.is_cuda and cov.dtype == torch.float64 and cov.is_contiguous()
+            and cov.dim() == 3 and cov.shape[1:] == (3, 3)):
+        raise MacvoB200Error("cov_modify: expects a contiguous (K,3,3) float64 CUDA tensor (modified in place)")
+    k = cov.shape[0]
+    if k and ops:
+        _check(load_library().macvo_cov_modify(cov.data_ptr(), k, C.cast(arr, C.c_void_p), len(ops), _stream()),
+               "macvo_cov_modify")
+        LAUNCHES[0] += 1
+    return cov
+
+
 def observe_pack(buf: ObservationBuffers, kp0_uv: Tensor, flow: Tensor, match_cov: Tensor, depth0: Tensor, depth1: Tensor,
                  disparity1: Tensor, disp_unc1: Tensor, edge_width: int, intr0, intr1, prev_pose: Tensor, next_pose: Tensor,
                  kernel_size: int = 31, min_flow_cov: float = 0.25, min_depth_cov: float = 0.05,
@@ -661,7 +689,8 @@ def observe_pack(buf: ObservationBuffers, kp0_uv: Tensor, flow: Tensor, match_co
 
     ext (None: CovarianceSanityFilter only) = macvo_observe_ext_t as a dict: depth_cov0 / depth_cov1 ((1,1,H,W) fp32 CUDA
     or None), simple_depth (bool), min_depth / max_depth (floats, rounded to fp32 like the reference's comparisons),
-    front_of_cam (bool), icp (bool: pack the "icp" graph's columns; needs an extended buffer)."""
+    front_of_cam (bool), icp (bool: pack the "icp" graph's columns; needs an extended buffer), cov_model ("match" or
+    "identity", the NoCovariance model) and cov_ops (modifier names of COV_OPS, innermost first)."""
     lib = load_library()
     kp = _dev(kp0_uv, torch.int64, "observe_pack kp0_uv")
     k = kp.shape[0]
@@ -680,7 +709,8 @@ def observe_pack(buf: ObservationBuffers, kp0_uv: Tensor, flow: Tensor, match_co
     i1 = (C.c_float * 4)(*[float(v) for v in intr1])
     xs = None
     if ext is not None:
-        unknown = set(ext) - {"depth_cov0", "depth_cov1", "simple_depth", "min_depth", "max_depth", "front_of_cam", "icp"}
+        unknown = set(ext) - {"depth_cov0", "depth_cov1", "simple_depth", "min_depth", "max_depth", "front_of_cam", "icp",
+                              "cov_model", "cov_ops"}
         if unknown:
             raise MacvoB200Error(f"observe_pack: unknown ext keys {sorted(unknown)}")
         if ext.get("icp") and not buf.extended:
@@ -691,6 +721,11 @@ def observe_pack(buf: ObservationBuffers, kp0_uv: Tensor, flow: Tensor, match_co
         xs = _ObserveExt(None if dc[0] is None else dc[0].data_ptr(), None if dc[1] is None else dc[1].data_ptr(),
                          int(bool(ext.get("simple_depth"))), float(ext.get("min_depth", 0.0)), float(ext.get("max_depth", 0.0)),
                          int(bool(ext.get("front_of_cam"))), int(bool(ext.get("icp"))))
+        model = ext.get("cov_model", "match")
+        if model not in COV_MODELS:
+            raise MacvoB200Error(f"observe_pack: cov_model must be one of {sorted(COV_MODELS)}, got {model!r}")
+        ops_ = tuple(ext.get("cov_ops", ()))
+        xs.cov_model, xs.cov_ops, xs.n_cov_ops = COV_MODELS[model], _cov_ops(ops_, "observe_pack"), len(ops_)
     buf.status.zero_()
     rc = lib.macvo_observe_pack(kp.data_ptr() if k else None, k, buf.capacity, fl.data_ptr(), mc.data_ptr(),
                                 *(m.data_ptr() for m in maps), H, W, int(edge_width), C.cast(i0, C.c_void_p),

@@ -217,7 +217,12 @@ class FusedTwoFrameOdometry:
     contains `B200_CovarianceSanityFilter`; the whole chain runs inside observe_pack (`plugins.observe_ext`). The graph
     type comes from `optimizer.context["graph_type"]`; "icp" packs its extra columns into the same buffer and the counted
     LM reads them there. Either `kp_selector` (B200_CovAwareSelector or its _NoDepth variant) is driven through
-    `enqueue_candidates`."""
+    `enqueue_candidates`.
+
+    The ablation back ends: `kp_selector` may be a B200_RandomSelector, whose keypoints are drawn on the device with no
+    candidate count, so that with mapping off a frame has NO host synchronisation (`host_waits` records each frame's
+    count). `cov_model` may be B200_NoCovariance or B200_Modifier_Diagonalize / _Normalize around a B200 model
+    (`plugins.cov_spec`): observe_pack applies the model, and the mapping branch gets the same covariances."""
 
     def __init__(self, frontend, kp_selector, cov_model, optimizer, num_point: int = 200, edgewidth: int = 32,
                  match_cov_default: float = 0.25, mapping: bool = True, map_selector=None, min_num_point: int = 10,
@@ -240,17 +245,28 @@ class FusedTwoFrameOdometry:
         self.mapping, self.min_num_point, self.num_map_point = mapping and map_selector is not None, min_num_point, num_map_point
         self.keep_debug = keep_debug
         self.device = kp_selector.device
-        cc = cov_model.config
-        self.cov_args = dict(kernel_size=cc.kernel_size, min_flow_cov=cc.min_flow_cov, min_depth_cov=cc.min_depth_cov)
+        from .plugins import B200_RandomSelector, cov_spec
+        self.random_kp = isinstance(kp_selector, B200_RandomSelector)   # drawn on the device: no candidate count to wait for
+        _, self.cov_ops, params = cov_spec(cov_model)
+        self.cov_identity = params is None
+        # B200_NoCovariance has no kernel parameters: observe_pack reads none of them then, and kernel_size 1 reduces the
+        # mapping branch's covariance kernel to the point gather at the centre pixel
+        self.cov_args = params or dict(kernel_size=1, min_flow_cov=0.25, min_depth_cov=0.05)
+        self.cov_ext = {}
+        if self.cov_identity or self.cov_ops:
+            self.cov_ext = {"cov_model": "identity" if self.cov_identity else "match", "cov_ops": list(self.cov_ops)}
         self.cluster = int(getattr(optimizer, "context", {}).get("cluster", 0)) if hasattr(optimizer, "context") else 0
         icp = self.graph_type == "icp"
         self.obs = [ops.ObservationBuffers(num_point, self.device, extended=icp) for _ in range(2)]      # double buffered
-        self.ext = None if outlier_filter is None and not icp else {}      # filled by initialize (set_meta resolves "auto")
+        # filled by initialize (set_meta resolves "auto")
+        self.ext = None if outlier_filter is None and not icp and not self.cov_ext else {}
+        self.host_waits: list[int] = []     # host synchronisations of each run_pair (0 or 1)
         self.stats = [torch.zeros((8,), dtype=torch.float64, device=self.device) for _ in range(2)]
         if self.mapping:
             self.map_cov = [torch.empty((num_map_point, 3, 3), dtype=torch.float64, device=self.device) for _ in range(2)]
             self.map_cov_host = [torch.empty((num_map_point, 3, 3), dtype=torch.float64).pin_memory() for _ in range(2)]
             self.map_pt_host = [torch.empty((num_map_point, 3), dtype=torch.float32).pin_memory() for _ in range(2)]
+            self._eye = torch.eye(3, dtype=torch.float64, device=self.device)
         self.pose_dev: list[torch.Tensor] = []          # (7,) float64 per frame, on the device
         self.pose_host = torch.zeros((2, 7), dtype=torch.float64).pin_memory()
         self.pose_ready = [torch.cuda.Event(), torch.cuda.Event()]
@@ -270,7 +286,7 @@ class FusedTwoFrameOdometry:
             from .plugins import observe_ext
             if self.outlier_filter is not None:
                 self.outlier_filter.set_meta(frame0)
-            self.ext = dict(observe_ext(self.outlier_filter) or {}, icp=self.graph_type == "icp")
+            self.ext = dict(observe_ext(self.outlier_filter) or {}, icp=self.graph_type == "icp", **self.cov_ext)
 
     @staticmethod
     def _intr(frame) -> tuple[float, float, float, float]:
@@ -297,26 +313,34 @@ class FusedTwoFrameOdometry:
         if self._tail_done is not None:            # the previous frame's tail read the candidate lists the selectors now overwrite
             main.wait_event(self._tail_done)
         # selection kernels for keypoints AND mapping points first, then a single synchronisation for both counts
-        reqs = [(self.kp_selector.enqueue_candidates(frame0, depth0, depth1, match01), self.num_point)]
+        # (B200_RandomSelector draws its keypoints right here, in frame order, and needs no count)
+        reqs, kp_random = [], None
+        if self.random_kp:
+            kp_random = self.kp_selector.select_device(frame0, self.num_point)
+        else:
+            reqs.append((self.kp_selector.enqueue_candidates(frame0, depth0, depth1, match01), self.num_point))
         if self.mapping:
             reqs.append((self.map_selector.enqueue_candidates(depth0), self.num_map_point))
         counts = ops.request_candidate_counts(reqs)
+        self.host_waits.append(1 if reqs else 0)
         if next_frame is None:
-            counts.synchronize()
-            return self._tail(frame0, frame1, depth0, depth1, match01, reqs, slot, fc1)
+            if reqs:
+                counts.synchronize()
+            return self._tail(frame0, frame1, depth0, depth1, match01, reqs, slot, fc1, kp_random)
         d_next, m_next = self.frontend.estimate_pair(frame1, next_frame)
         self._prefetched = (next_frame, d_next, m_next, self._enqueue_motion(next_frame, d_next, m_next))
-        counts.synchronize()
+        if reqs:
+            counts.synchronize()
         if self._tail_stream is None:
             self._tail_stream = torch.cuda.Stream(self.device)
         tail = self._tail_stream
         tail.wait_event(counts)
         for t in (match01.flow, match01.cov, depth0.depth, depth1.depth, depth1.disparity, depth1.disparity_uncertainty, fc1,
-                  depth0.cov, depth1.cov):
+                  depth0.cov, depth1.cov, kp_random):
             if t is not None:
                 t.record_stream(tail)          # allocated on the main stream, consumed on the tail stream
         with torch.cuda.stream(tail):
-            res = self._tail(frame0, frame1, depth0, depth1, match01, reqs, slot, fc1)
+            res = self._tail(frame0, frame1, depth0, depth1, match01, reqs, slot, fc1, kp_random)
             self._tail_done = torch.cuda.Event()
             self._tail_done.record(tail)
         return res
@@ -328,10 +352,12 @@ class FusedTwoFrameOdometry:
             return None
         return self.motion_model.enqueue(frame1, match01.flow, depth1.depth).clone()
 
-    def _tail(self, frame0, frame1, depth0, depth1, match01, reqs, slot, fc1=None) -> FrameResult:
+    def _tail(self, frame0, frame1, depth0, depth1, match01, reqs, slot, fc1=None, kp_random=None) -> FrameResult:
         """everything after the candidate counts reached the host, on the current stream"""
         ops = self.ops
         picks = ops.sample_from_counts(reqs)
+        if kp_random is not None:
+            picks.insert(0, kp_random)
         kp0_uv = picks[0]
         obs, stats = self.obs[slot], self.stats[slot]
         next_pose = torch.empty((7,), dtype=torch.float64, device=self.device)
@@ -362,6 +388,10 @@ class FusedTwoFrameOdometry:
                                                 min_flow_cov=self.cov_args["min_flow_cov"],
                                                 min_depth_cov=self.cov_args["min_depth_cov"], match_cov_default=sig,
                                                 want_point=True, out_cov=self.map_cov[slot][:n_map])
+                if self.cov_identity:   # NoCovariance: the covariances are the identity, the points as above
+                    self.map_cov[slot][:n_map].copy_(self._eye.expand(n_map, 3, 3))
+                if self.cov_ops:
+                    ops.cov_modify(self.map_cov[slot][:n_map], self.cov_ops)
                 self.map_cov_host[slot][:n_map].copy_(self.map_cov[slot][:n_map], non_blocking=True)
                 self.map_pt_host[slot][:n_map].copy_(pt, non_blocking=True)
         self.n_map[slot] = n_map

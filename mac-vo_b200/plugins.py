@@ -4,7 +4,11 @@
     B200_CovAwareSelector_NoDepth    IKeypointSelector  replaces CovAwareSelector_NoDepth (KeypointSelector.py:349-407)
     B200_CovAwareSelector            IKeypointSelector  replaces CovAwareSelector (KeypointSelector.py:250-347)
     B200_MappingPointSelector        IKeypointSelector  replaces MappingPointSelector (KeypointSelector.py:78-100)
+    B200_RandomSelector              IKeypointSelector  replaces RandomSelector (KeypointSelector.py:103-118)
     B200_MatchCovariance             ICovariance2to3    replaces MatchCovariance (Covariance/Project2to3.py:114-182)
+    B200_NoCovariance                ICovariance2to3    replaces NoCovariance (Covariance/Project2to3.py:48-57)
+    B200_Modifier_Diagonalize        ICovariance2to3    replaces Modifier_Diagonalize (Covariance/Project2to3.py:281-302)
+    B200_Modifier_Normalize          ICovariance2to3    replaces Modifier_Normalize (Covariance/Project2to3.py:305-323)
     B200_CovarianceSanityFilter      IObservationFilter replaces CovarianceSanityFilter (OutlierFilter.py:91-100)
     B200_SimpleDepthFilter           IObservationFilter replaces SimpleDepthFilter (OutlierFilter.py:103-124)
     B200_LikelyFrontOfCamFilter      IObservationFilter replaces LikelyFrontOfCamFilter (OutlierFilter.py:127-141)
@@ -327,6 +331,35 @@ class B200_CovAwareSelector(IKeypointSelector):
         })
 
 
+class B200_RandomSelector(IKeypointSelector):
+    """Replacement of RandomSelector.select_point (KeypointSelector.py:103-118), the selector of the CovOpt ablation:
+    `numPoint` uniform (u, v) in [mask_width, size - mask_width), duplicates possible, drawn by the reference's two
+    `torch.randint` calls (rows, then columns) on the configured CUDA device's generator — the same Philox stream, so the
+    same keypoints from the same generator state. No candidate list and no host synchronisation."""
+
+    def __init__(self, config: SimpleNamespace):
+        super().__init__(config)
+        self.device = _require_cuda(config.device, "B200_RandomSelector")
+
+    def select_device(self, frame, numPoint: int) -> torch.Tensor:
+        """(numPoint, 2) int64 on the device; kernels only (what the fused driver calls)"""
+        mw = self.config.mask_width
+        h_indices = torch.randint(mw, frame.height - mw, (numPoint, 1), device=self.device)
+        w_indices = torch.randint(mw, frame.width - mw, (numPoint, 1), device=self.device)
+        return torch.cat([w_indices, h_indices], dim=1)
+
+    @torch.inference_mode()
+    def select_point(self, frame, numPoint: int, depth0_est, depth1_est, match_est) -> torch.Tensor:
+        return self.select_device(frame, numPoint)
+
+    @classmethod
+    def is_valid_config(cls, config: SimpleNamespace | None) -> None:
+        cls._enforce_config_spec(config, {
+            "mask_width": lambda m: isinstance(m, int) and m >= 0,
+            "device": lambda dev: isinstance(dev, str) and "cuda" in dev,
+        })
+
+
 class B200_MappingPointSelector(IKeypointSelector):
     """Bit-exact replacement of MappingPointSelector.select_point (KeypointSelector.py:87-100)."""
 
@@ -396,6 +429,11 @@ class B200_MatchCovariance(ICovariance2to3):
     @torch.inference_mode()
     def estimate(self, frame, kp, depth_est, depth_cov, flow_cov) -> torch.Tensor:
         cov, _ = self.estimate_device(frame, kp, depth_est, depth_cov, flow_cov)
+        return self.download(cov)
+
+    def download(self, cov: torch.Tensor) -> torch.Tensor:
+        """the CPU float64 copy of `estimate_device`'s covariances (or of a modified version of them); raises the
+        reference's IndexError when the last estimate's depth patch left the image"""
         if self._status_host is None:
             self._status_host = torch.zeros((1,), dtype=self.last_status.dtype).pin_memory()
         self._status_host.copy_(self.last_status, non_blocking=True)      # rides in front of the blocking copy below
@@ -413,6 +451,98 @@ class B200_MatchCovariance(ICovariance2to3):
             "min_depth_cov": lambda c: isinstance(c, (int, float)) and c > 0,
             "min_flow_cov": lambda c: isinstance(c, (int, float)) and c > 0,
         })
+
+
+class B200_NoCovariance(ICovariance2to3):
+    """Replacement of NoCovariance (Project2to3.py:48-57), the covariance model of the CovKP ablation: identity
+    covariances. Like the reference it reads no depth patch and leaves `flow_cov` alone, so the MatchObs column
+    `pixel2_uv_cov` keeps the network's unclamped values. config: none."""
+
+    def estimate(self, frame, kp, depth_est, depth_cov, flow_cov) -> torch.Tensor:
+        return torch.eye(3).unsqueeze(0).repeat(kp.size(0), 1, 1).double()       # CPU float64, as the reference
+
+    def estimate_device(self, frame, kp, depth_est, depth_cov, flow_cov, want_point: bool = False):
+        """(identity (K,3,3) float64 on the keypoints' / depth map's device, None). The fused driver does not call this:
+        observe_pack and its mapping branch build the identity themselves."""
+        if want_point:
+            raise ValueError("B200_NoCovariance.estimate_device computes no points")
+        dev = kp.device if kp.is_cuda else depth_est.depth.device
+        return torch.eye(3, dtype=torch.float64, device=dev).repeat(kp.size(0), 1, 1), None
+
+    def download(self, cov: torch.Tensor) -> torch.Tensor:
+        return cov.cpu()
+
+    @classmethod
+    def is_valid_config(cls, config: SimpleNamespace | None) -> None:
+        return
+
+
+class _B200_CovModifier(ICovariance2to3):
+    """A modifier wrapping another B200 covariance model (config: `type` / `args` of the nested model), applied on the
+    device by `macvo_cov_modify`."""
+    OP = ""
+
+    def __init__(self, config: SimpleNamespace):
+        super().__init__(config)
+        _require_b200_cov(config.type, type(self).__name__)
+        self.submodule = ICovariance2to3.instantiate(config.type, config.args)
+
+    def estimate_device(self, frame, kp, depth_est, depth_cov, flow_cov, want_point: bool = False):
+        cov, pt = self.submodule.estimate_device(frame, kp, depth_est, depth_cov, flow_cov, want_point=want_point)
+        return ops.cov_modify(cov, [self.OP]), pt
+
+    @torch.inference_mode()
+    def estimate(self, frame, kp, depth_est, depth_cov, flow_cov) -> torch.Tensor:
+        cov, _ = self.estimate_device(frame, kp, depth_est, depth_cov, flow_cov)
+        return self.download(cov)
+
+    def download(self, cov: torch.Tensor) -> torch.Tensor:
+        return self.submodule.download(cov)
+
+    @classmethod
+    def is_valid_config(cls, config: SimpleNamespace | None) -> None:
+        assert config is not None
+        _require_b200_cov(getattr(config, "type", None), cls.__name__)
+        ICovariance2to3.is_valid_config(config)
+
+
+class B200_Modifier_Diagonalize(_B200_CovModifier):
+    """Replacement of Modifier_Diagonalize (Project2to3.py:281-302): the nested model's covariances with their six
+    off-diagonal entries set to 0 (a NaN / Inf there disappears before CovarianceSanityFilter sees it)."""
+    OP = "diagonalize"
+
+
+class B200_Modifier_Normalize(_B200_CovModifier):
+    """Replacement of Modifier_Normalize (Project2to3.py:305-323): each covariance divided by its OWN determinant (3x3 LU
+    with partial pivoting in float64; det 0 gives +-Inf / NaN, which the sanity filter drops, a negative det flips the
+    matrix's sign)."""
+    OP = "normalize"
+
+
+def _require_b200_cov(name, who: str) -> None:
+    try:
+        cls = ICovariance2to3.get_class(name)
+    except (KeyError, TypeError):
+        cls = None
+    if not (isinstance(cls, type) and issubclass(cls, (B200_MatchCovariance, B200_NoCovariance, _B200_CovModifier))):
+        raise ValueError(f"{who}: the nested covariance model must be a B200 model (B200_MatchCovariance, "
+                         f"B200_NoCovariance or another B200 modifier), got {name!r}")
+
+
+def cov_spec(cov_model) -> tuple[ICovariance2to3, list[str], dict | None]:
+    """(base model, modifiers innermost first, the base model's kernel parameters or None for B200_NoCovariance) of a
+    B200 covariance model: what `macvo_observe_pack` and the fused driver's mapping branch need."""
+    ops_: list[str] = []
+    m = cov_model
+    while isinstance(m, _B200_CovModifier):
+        ops_.insert(0, m.OP)
+        m = m.submodule
+    if isinstance(m, B200_NoCovariance):
+        return m, ops_, None
+    if isinstance(m, B200_MatchCovariance):
+        c = m.config
+        return m, ops_, dict(kernel_size=c.kernel_size, min_flow_cov=c.min_flow_cov, min_depth_cov=c.min_depth_cov)
+    raise ValueError(f"{type(m).__name__} has no device implementation in the fused driver")
 
 
 # ================================================================================================
@@ -808,6 +938,10 @@ PLUGINS = {
     "keypoint_depth": B200_CovAwareSelector,
     "mappoint": B200_MappingPointSelector,
     "cov": B200_MatchCovariance,
+    "cov_none": B200_NoCovariance,
+    "cov_diagonalize": B200_Modifier_Diagonalize,
+    "cov_normalize": B200_Modifier_Normalize,
+    "keypoint_random": B200_RandomSelector,
     "outlier": B200_CovarianceSanityFilter,
     "postprocess": B200_MotionInterpolate,
     "optimizer": B200_TwoFrame_PGO,
