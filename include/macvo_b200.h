@@ -283,6 +283,16 @@ int macvo_add_layer_norm(const float* x, const float* resid, const float* weight
  * operands; w1 / w2 are truncated by the MMA, so pass them pre-rounded the same way to compute what cuBLAS TF32 computes. */
 int macvo_mlp_tc(const float* xn, const float* resid, const float* w1, const float* b1, const float* w2, const float* b2,
                  float* out, int rows, int channels, int hidden, void* stream);
+/* PatchEmbed token head in one TF32 tensor-core kernel:
+ *     out[r] = LayerNorm(w2 relu(w0 x[r] + term[r % period]) + b2; ln_w, ln_b, eps)
+ * x (rows, in_channels), out (rows, channels) contiguous; w0 (channels, in_channels), term (period, channels),
+ * w2 (channels, channels), b2 / ln_w / ln_b (channels); in_channels == 64, channels == 128 (else MACVO_E_UNSUPPORTED);
+ * every pointer 16-byte aligned; out may not alias x. x and the hidden activation are rounded to tf32, nearest-even, as
+ * cuBLAS rounds TF32 GEMM operands; pass w0 / w2 pre-rounded the same way to compute what the cuBLAS TF32 GEMMs, the
+ * bias + ReLU pass and macvo_layer_norm compute, bit for bit. */
+int macvo_patch_tokens_tc(const float* x, const float* w0, const float* term, const float* w2, const float* b2,
+                          const float* ln_w, const float* ln_b, float* out, long long rows, int in_channels, int channels,
+                          int period, float eps, void* stream);
 /* maps (n_maps, 1, h, w) -> out (n_maps, ho, wo, 16) [NHWC], ho = ceil8(h)/2, wo = ceil8(w)/2:
  * ReLU(conv2d(zero-pad to multiples of 8, weight (16,1,6,6), stride 2, padding 2) + bias).
  * allow_tf32 bit 0: TF32 tensor-core implicit GEMM (what cuDNN does for the reference under cudnn.allow_tf32), else fp32 FMA.

@@ -19,7 +19,8 @@ LIB_DIR = os.path.join(PKG_DIR, "lib")
 LIB_PATH = os.path.join(LIB_DIR, "libmacvo_b200.so")
 SOURCES = ["corr_build.cu", "corr_build_simt.cu", "corr_build_tc.cu", "corr_lookup.cu", "dense_select.cu",
            "cov2to3.cu", "pgo.cu", "nn_kernels.cu", "decoder_fused.cu", "observe.cu", "decoder_token.cu", "motion_interp.cu",
-           "gru_conv_tc.cu", "conv_tc.cu", "posenet.cu", "mlp_tc.cu"]
+           "gru_conv_tc.cu", "conv_tc.cu", "posenet.cu", "mlp_tc.cu",
+           "patch_tokens_tc.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "--use_fast_math=false"]
 

@@ -11,6 +11,7 @@
 // core/attention.py:6-29, core/twins.py:103-114,173-183, core/Twins/svt_large.py:111-114,161-164); numerics:
 // fp32 throughout, exact erf-free ops only, parity vs torch fp32 in tests/test_gpu_nn_kernels.py.
 #include "common.cuh"
+#include "layer_norm_row.cuh"
 #include <math_constants.h>
 
 namespace {
@@ -31,7 +32,6 @@ layer_norm_kernel(const float* __restrict__ x, const float* __restrict__ w, cons
     if (row >= rows) return;
     const float* xr = x + row * C;
     float v[VPL];
-    float s = 0.f;
 #pragma unroll
     for (int i = 0; i < VPL / 4; ++i) {                           // lane owns float4 chunks lane + 32 i
         float4 t = *reinterpret_cast<const float4*>(xr + (lane + 32 * i) * 4);
@@ -41,25 +41,12 @@ layer_norm_kernel(const float* __restrict__ x, const float* __restrict__ w, cons
             *reinterpret_cast<float4*>(sum_out + row * C + (lane + 32 * i) * 4) = t;
         }
         v[4 * i] = t.x; v[4 * i + 1] = t.y; v[4 * i + 2] = t.z; v[4 * i + 3] = t.w;
-        s += (t.x + t.y) + (t.z + t.w);
     }
-    const float mean = warp_sum(s) * (1.f / C);
-    float q = 0.f;
-#pragma unroll
-    for (int i = 0; i < VPL; ++i) { const float d = v[i] - mean; q = fmaf(d, d, q); }
-    const float rstd = rsqrtf(warp_sum(q) * (1.f / C) + eps);
+    layer_norm_row<VPL>(v, w, b, eps, lane);
     float* yr = y + row * C;
 #pragma unroll
-    for (int i = 0; i < VPL / 4; ++i) {
-        const int c = (lane + 32 * i) * 4;
-        const float4 ww = *reinterpret_cast<const float4*>(w + c), bb = *reinterpret_cast<const float4*>(b + c);
-        float4 o;
-        o.x = (v[4 * i] - mean) * rstd * ww.x + bb.x;
-        o.y = (v[4 * i + 1] - mean) * rstd * ww.y + bb.y;
-        o.z = (v[4 * i + 2] - mean) * rstd * ww.z + bb.z;
-        o.w = (v[4 * i + 3] - mean) * rstd * ww.w + bb.w;
-        *reinterpret_cast<float4*>(yr + c) = o;
-    }
+    for (int i = 0; i < VPL / 4; ++i)
+        *reinterpret_cast<float4*>(yr + (lane + 32 * i) * 4) = make_float4(v[4 * i], v[4 * i + 1], v[4 * i + 2], v[4 * i + 3]);
 }
 
 // C = 64: two channels per lane

@@ -475,9 +475,16 @@ class FlowFormerCovNet:
             return term.contiguous()
         term = self._memo(("pe", h, w, x.dtype, x.device, native), coord_term)
         t = x.permute(0, 2, 3, 1).reshape(M, h * w, COST_INPUT_DIM)                        # tokens (free view in NHWC)
+        w2 = self.W[p + "ffn_with_coord.2.weight"][:, :, 0, 0]
+        if native and torch.backends.cuda.matmul.allow_tf32:
+            # linear, add_rows_relu_, linear, LayerNorm in one kernel (csrc/patch_tokens_tc.cu) with the same bits
+            w0t, w2t = self._memo(("pe_tc", x.device), lambda: (self._ops.round_tf32(w0[:, :COST_INPUT_DIM, 0, 0]),
+                                                                self._ops.round_tf32(w2)))
+            return self._ops.patch_tokens_tc(t, w0t, term[0], w2t, self.W[p + "ffn_with_coord.2.bias"],
+                                             self.W[p + "norm.weight"], self.W[p + "norm.bias"])
         t = F.linear(t, w0[:, :COST_INPUT_DIM, 0, 0])
         t = self._ops.add_rows_relu_(t, term[0]) if native else F.relu(t + term)
-        t = F.linear(t, self.W[p + "ffn_with_coord.2.weight"][:, :, 0, 0], self.W[p + "ffn_with_coord.2.bias"])
+        t = F.linear(t, w2, self.W[p + "ffn_with_coord.2.bias"])
         return self._ln(t, p + "norm")
 
     def _latent_layer(self, x: Tensor, p: str) -> Tensor:

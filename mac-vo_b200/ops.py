@@ -96,6 +96,7 @@ EXPORTS = {
     "macvo_layer_norm": (C.c_int, [C.c_void_p] * 4 + [C.c_longlong, C.c_int, C.c_float, C.c_void_p]),
     "macvo_add_layer_norm": (C.c_int, [C.c_void_p] * 6 + [C.c_longlong, C.c_int, C.c_float, C.c_void_p]),
     "macvo_mlp_tc": (C.c_int, [C.c_void_p] * 7 + [C.c_int] * 3 + [C.c_void_p]),
+    "macvo_patch_tokens_tc": (C.c_int, [C.c_void_p] * 8 + [C.c_longlong, C.c_int, C.c_int, C.c_int, C.c_float, C.c_void_p]),
     "macvo_patch_embed_conv1": (C.c_int, [C.c_void_p] * 4 + [C.c_longlong, C.c_int, C.c_int, C.c_int, C.c_void_p]),
     "macvo_add_rows_relu": (C.c_int, [C.c_void_p] * 2 + [C.c_longlong, C.c_int, C.c_int, C.c_void_p]),
     "macvo_small_attention": (C.c_int, [C.c_void_p] * 4 + [C.c_int] * 7 + [C.c_void_p]),
@@ -887,6 +888,29 @@ def mlp_tc(xn: Tensor, resid: Tensor, w1: Tensor, b1: Tensor, w2: Tensor, b2: Te
     rc = load_library().macvo_mlp_tc(xn.data_ptr(), resid.data_ptr(), w1.data_ptr(), b1.data_ptr(), w2.data_ptr(),
                                       b2.data_ptr(), out.data_ptr(), xn.numel() // c, c, hd, _stream())
     _check(rc, "macvo_mlp_tc")
+    LAUNCHES[0] += 1
+    return out
+
+
+def patch_tokens_tc(x: Tensor, w0: Tensor, term: Tensor, w2: Tensor, b2: Tensor, ln_w: Tensor, ln_b: Tensor,
+                    eps: float = 1e-5) -> Tensor:
+    """LayerNorm(w2 relu(w0 x + term[row % period]) + b2) over the last dim of x (..., 64) -> (..., 128) in one TF32
+    tensor-core kernel (csrc/patch_tokens_tc.cu): PatchEmbed's token head. With w0 / w2 from `round_tf32` it returns the
+    bits of cuBLAS TF32 linear, add_rows_relu_, cuBLAS TF32 linear + bias and layer_norm."""
+    x, term = _dev(x, torch.float32, "patch_tokens_tc x"), _dev(term, torch.float32, "patch_tokens_tc term")
+    w0, w2 = _dev(w0, torch.float32, "patch_tokens_tc w0"), _dev(w2, torch.float32, "patch_tokens_tc w2")
+    b2 = _dev(b2, torch.float32, "patch_tokens_tc b2")
+    ln_w, ln_b = _dev(ln_w, torch.float32, "patch_tokens_tc ln_w"), _dev(ln_b, torch.float32, "patch_tokens_tc ln_b")
+    cin, c = x.shape[-1], w0.shape[0]
+    if (cin != 64 or c != 128 or tuple(w0.shape) != (c, cin) or tuple(w2.shape) != (c, c) or term.dim() != 2
+            or term.shape[1] != c or term.shape[0] == 0 or any(t.numel() != c for t in (b2, ln_w, ln_b))):
+        raise MacvoB200Error(f"patch_tokens_tc: unsupported shapes x {tuple(x.shape)}, w0 {tuple(w0.shape)}, "
+                             f"term {tuple(term.shape)}, w2 {tuple(w2.shape)}")
+    out = torch.empty(*x.shape[:-1], c, dtype=torch.float32, device=x.device)
+    rc = load_library().macvo_patch_tokens_tc(x.data_ptr(), w0.data_ptr(), term.data_ptr(), w2.data_ptr(), b2.data_ptr(),
+                                              ln_w.data_ptr(), ln_b.data_ptr(), out.data_ptr(), x.numel() // cin, cin, c,
+                                              term.shape[0], float(eps), _stream())
+    _check(rc, "macvo_patch_tokens_tc")
     LAUNCHES[0] += 1
     return out
 
