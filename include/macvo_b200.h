@@ -97,6 +97,10 @@ int macvo_corr_lookup_rows(const float* cost_maps, const float* coords, float* o
  * `score->nms` (h*w uint8) = quality == min over the ksize x ksize window and no NaN in it;
  * NMS survivors' quality values are appended (unordered) to score->cand_vals, count in *score->n_cand
  * (caller zeroes it). All pointers device memory.
+ * est_cov == NULL with est_flow set: a frontend without covariance (FlowFormerDepth.estimate,
+ * Module/Frontend/StereoDepth.py:122-128: disparity = |flow_x| of slot 0, depth = (bl*fx) * disparity.reciprocal(),
+ * StereoDepth.py:270-272). Only depth and / or disparity are written, with the arithmetic above; depth_cov,
+ * depth_mask, flow_cov and score must be NULL (MACVO_E_ARG otherwise).
  */
 typedef struct {
     const float* score_cov; /* (3,h,w) or NULL = use the freshly written flow_cov */
@@ -469,6 +473,14 @@ int macvo_observe_pack(const int64_t* kp0_uv, int k, int capacity, const float* 
                        float min_flow_cov, float min_depth_cov, float match_cov_default, const double* prev_pose,
                        double* next_pose, double* packed, int* n_obs, int* status, void* workspace,
                        size_t workspace_bytes, void* stream, const macvo_observe_ext_t* ext);
+/* match_cov == NULL && disp_unc1 == NULL: the frontend gives no covariance maps (FrontendCompose of FlowFormerDepth +
+ * FlowFormerMatcher, the Vanilla ablation; Odometry/MACVO.py:212-264 with kp*_sigma_dd, kp1_sigma_disparity and
+ * kp1_sigma_uv None). Passing only one of the two as NULL is MACVO_E_ARG.
+ *   - pixel2_uv_cov (all 3 columns) and pixel2_disp_cov hold -1, MatchObs' placeholder (MACVO.py:250-264); so do the
+ *     icp columns pixel1_d_cov / pixel2_d_cov when ext->depth_cov0 / depth_cov1 are NULL, as above.
+ *   - MACVO_COV_MATCH: MatchCovariance.estimate with flow_cov None for kp1 (Project2to3.py:128-135): its 2x2 flow
+ *     covariance is match_cov_default * [1, 1, 0] WITHOUT the min_flow_cov^2 clamp; kp0 keeps the clamped default.
+ *   - MACVO_COV_IDENTITY: unchanged (identity covariances). */
 
 /* ------------------------------------------------------------------------------------------------
  * (f2) decoder token path of one refinement iteration as one kernel — replaces flow_token_encoder (decoder.py:112-116),

@@ -34,13 +34,15 @@ dense_score_kernel(const float* __restrict__ est_flow, const float* __restrict__
     const int p = y * w + x;
 
     // ---- (a7) slot 0: disparity -> depth, depth covariance ------------------------------------
+    // (est_cov == nullptr: a frontend without covariance, FlowFormerDepth.estimate, StereoDepth.py:122-128 -- depth and
+    // disparity only)
     if (inside && est_flow != nullptr) {
         const float fxv = est_flow[p];                       // est_flow[0, 0]
-        const float dcv = est_cov[p];                        // est_cov[0, 0]  (disparity variance)
         const float disp = fabsf(fxv);
         if (disparity) disparity[p] = disp;
         if (depth) depth[p] = __fmul_rn(bl_fx, __frcp_rn(disp));
         if (depth_cov) {
+            const float dcv = est_cov[p];                    // est_cov[0, 0]  (disparity variance)
             const float d2 = __fmul_rn(disp, disp);
             const float err2 = __fmul_rn(dcv, __frcp_rn(d2));
             depth_cov[p] = __fmul_rn(bl_fx_sq, __fdiv_rn(err2, d2));
@@ -49,7 +51,7 @@ dense_score_kernel(const float* __restrict__ est_flow, const float* __restrict__
     }
     // ---- slot 1: match covariance, padded to 3 channels with zeros -----------------------------
     float cuu = 0.f, cvv = 0.f, cuv = 0.f;
-    if (inside) {
+    if (inside && (score_cov || est_cov)) {
         if (score_cov) {
             cuu = score_cov[p]; cvv = score_cov[hw + p]; cuv = score_cov[2 * hw + p];
         } else {
@@ -271,8 +273,13 @@ extern "C" int macvo_dense_postproc(const float* est_flow, const float* est_cov,
                                     double bl_fx_sq, float* depth, float* disparity, float* depth_cov,
                                     uint8_t* depth_mask, float* flow_cov, const macvo_score_t* score, void* stream) {
     if (h <= 0 || w <= 0) return MACVO_E_ARG;
-    if (!est_cov && !(score && score->score_cov)) return MACVO_E_ARG;
-    if ((depth || disparity || depth_cov || depth_mask) && (!est_flow || !est_cov)) return MACVO_E_ARG;
+    if (!est_cov && est_flow) {
+        // no covariance maps: depth / disparity of slot 0 only (FlowFormerDepth.estimate)
+        if (depth_cov || depth_mask || flow_cov || score || !(depth || disparity)) return MACVO_E_ARG;
+    } else if (!est_cov && !(score && score->score_cov)) {
+        return MACVO_E_ARG;
+    }
+    if ((depth || disparity || depth_cov || depth_mask) && !est_flow) return MACVO_E_ARG;
     int radius = 0;
     const float* score_cov = nullptr;
     float* quality = nullptr; uint8_t* nms = nullptr; float* cand = nullptr; int* ncand = nullptr;

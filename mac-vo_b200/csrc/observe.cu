@@ -26,11 +26,11 @@ struct ObserveArgs {
     const int64_t* kp0;            // (k,2) [u,v] selected keypoints on frame 0
     int k;
     const float* flow;             // (2,h,w) match flow frame0 -> frame1
-    const float* match_cov;        // (3,h,w) [uu, vv, uv]
+    const float* match_cov;        // (3,h,w) [uu, vv, uv], or nullptr with disp_unc1: a frontend without covariance
     const float* depth0;           // (h,w)
     const float* depth1;           // (h,w)
     const float* disparity1;       // (h,w)
-    const float* disp_unc1;        // (h,w)
+    const float* disp_unc1;        // (h,w) or nullptr
     int h, w, edge;
     macvo::CovParams P0, P1;       // intrinsics of frame 0 / frame 1 + covariance-model parameters
     float min_flow_var, match_cov_default;
@@ -158,10 +158,12 @@ observe_kernel(ObserveArgs A, float* __restrict__ rec, int* __restrict__ status)
     const long long ul1 = (long long)u1, vl1 = (long long)v1;         // .long(): truncation
     const int p1 = (int)(vl1 * A.w + ul1);                            // inside the image: edge > 0
     const float d0 = A.depth0[p0];
-    const float disp1 = A.disparity1[p1], dunc1 = A.disp_unc1[p1];
+    // no covariance maps (MACVO.py:250-264): MatchObs holds the -1 placeholder in pixel2_uv_cov and pixel2_disp_cov
+    const bool no_cov = A.match_cov == nullptr;
+    const float disp1 = A.disparity1[p1], dunc1 = no_cov ? -1.f : A.disp_unc1[p1];
     float c0[6], c1[6];
-    const float a = A.match_cov[p0], b = A.match_cov[hw + p0];
-    const float suv = A.match_cov[2 * hw + p0];
+    const float a = no_cov ? -1.f : A.match_cov[p0], b = no_cov ? -1.f : A.match_cov[hw + p0];
+    const float suv = no_cov ? -1.f : A.match_cov[2 * hw + p0];
     float suu, svv;
     bool oob = false;
     if (A.identity) {
@@ -174,10 +176,18 @@ observe_kernel(ObserveArgs A, float* __restrict__ rec, int* __restrict__ status)
         // frame-0 keypoints: constant quantisation covariance, clamped like any flow_cov (Project2to3.py:130-133)
         const float s0 = fmaxf(A.match_cov_default, A.min_flow_var);
         oob = macvo::match_cov_warp((float)u0, (float)v0, u0, v0, A.depth0, A.h, A.w, s0, s0, 0.f, false, 0.f, A.P0, lane, c0);
-        // frame-1 keypoints: the network's match covariance at the source pixel, clamped in place
-        suu = (a != a) ? a : fmaxf(a, A.min_flow_var);
-        svv = (b != b) ? b : fmaxf(b, A.min_flow_var);
-        oob |= macvo::match_cov_warp(u1, v1, ul1, vl1, A.depth1, A.h, A.w, suu, svv, suv, false, 0.f, A.P1, lane, c1);
+        if (no_cov) {
+            // frame-1 keypoints without a network covariance: MatchCovariance's own default, NOT clamped
+            // (Project2to3.py:128-135); the packed column keeps the placeholder
+            const float s1 = A.match_cov_default;
+            oob |= macvo::match_cov_warp(u1, v1, ul1, vl1, A.depth1, A.h, A.w, s1, s1, 0.f, false, 0.f, A.P1, lane, c1);
+            suu = svv = -1.f;
+        } else {
+            // frame-1 keypoints: the network's match covariance at the source pixel, clamped in place
+            suu = (a != a) ? a : fmaxf(a, A.min_flow_var);
+            svv = (b != b) ? b : fmaxf(b, A.min_flow_var);
+            oob |= macvo::match_cov_warp(u1, v1, ul1, vl1, A.depth1, A.h, A.w, suu, svv, suv, false, 0.f, A.P1, lane, c1);
+        }
         if (lane != 0) return;
     }
     if (oob) atomicOr(status, 1);                // status is a bitmask: both conditions may occur in one call
@@ -421,7 +431,9 @@ extern "C" int macvo_observe_pack(const int64_t* kp0_uv, int k, int capacity, co
     if (k < 0 || capacity < 1 || k > capacity || h <= 0 || w <= 0 || edge_width <= 0 || kernel_size < 1 ||
         (kernel_size & 1) == 0 || kernel_size > 31)
         return MACVO_E_ARG;
-    if (!flow || !match_cov || !depth0 || !depth1 || !disparity1 || !disp_unc1 || !intr0 || !intr1 || !prev_pose ||
+    // match_cov and disp_unc1 are NULL together (a frontend without covariance) or not at all
+    if (!match_cov != !disp_unc1) return MACVO_E_ARG;
+    if (!flow || !depth0 || !depth1 || !disparity1 || !intr0 || !intr1 || !prev_pose ||
         !next_pose || !packed || !n_obs || !status || !workspace || (k > 0 && !kp0_uv))
         return MACVO_E_ARG;
     if (workspace_bytes < macvo_observe_workspace_bytes(capacity)) return MACVO_E_WORKSPACE;

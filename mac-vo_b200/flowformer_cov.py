@@ -104,8 +104,12 @@ def _gru_spec(p: str) -> list[tuple[str, tuple[int, ...], str]]:
     return out
 
 
-def param_spec() -> list[tuple[str, tuple[int, ...], str]]:
-    """All 428 tensors of the reference `FlowFormerCov.state_dict()` (SURVEY.md Appendix A)."""
+COV_PREFIX = "memory_decoder.cov_update."
+
+
+def param_spec(covariance: bool = True) -> list[tuple[str, tuple[int, ...], str]]:
+    """All 428 tensors of the reference `FlowFormerCov.state_dict()` (SURVEY.md Appendix A); with covariance=False the
+    plain FlowFormer's (core/transformer.py): the same keys without the covariance decoder's `cov_update.*`."""
     D = LATENT_DIM
     s = _svt_spec("memory_encoder.feat_encoder")
     s += [("memory_encoder.channel_convertor.weight", (256, 256, 1, 1), "w")]
@@ -167,10 +171,10 @@ def param_spec() -> list[tuple[str, tuple[int, ...], str]]:
           (m + "cov_update.mask.0.weight", (256, 128, 3, 3), "w"), (m + "cov_update.mask.0.bias", (256,), "b"),
           (m + "cov_update.mask.2.weight", (576, 256, 1, 1), "w"), (m + "cov_update.mask.2.bias", (576,), "b")]
     s += _svt_spec("context_encoder")
-    return s
+    return s if covariance else [e for e in s if not e[0].startswith(COV_PREFIX)]
 
 
-def synthetic_state_dict(seed: int = 0) -> dict[str, Tensor]:
+def synthetic_state_dict(seed: int = 0, covariance: bool = True) -> dict[str, Tensor]:
     """Deterministic stand-in for the released checkpoint (absent: no network, SURVEY.md §8c).
 
     Every tensor is drawn from its own generator seeded by (seed, crc32(key)), so the values do not
@@ -178,9 +182,10 @@ def synthetic_state_dict(seed: int = 0) -> dict[str, Tensor]:
     (`tests/golden/make_golden.py`) — that is how the golden fixtures are tied to these weights.
     Weights ~ U(+-1/sqrt(fan_in)) (torch's default conv/linear init), norms (1, 0), GMA gamma 0.5
     (the reference initialises it to 0, which would leave the aggregation path untested).
+    covariance=False: the plain FlowFormer's tensors, each with the same values as in the covariance variant.
     """
     sd: dict[str, Tensor] = {}
-    for key, shape, kind in param_spec():
+    for key, shape, kind in param_spec(covariance):
         g = torch.Generator().manual_seed((seed * 1000003 + zlib.crc32(key.encode())) % (2 ** 31))
         if kind == "one":
             t = torch.ones(shape)
@@ -239,14 +244,21 @@ def _sdpa(q: Tensor, k: Tensor, v: Tensor) -> Tensor:
 
 
 class FlowFormerCovNet:
-    """Functional FlowFormerCov. `inference(image1, image2) -> (flow, cov)` like flownet.py:37-44."""
+    """Functional FlowFormerCov. `inference(image1, image2) -> (flow, cov)` like flownet.py:37-44.
+
+    covariance=False builds the plain FlowFormer (core/transformer.py, core/decoder.py:155-203): the covariance decoder's
+    flow track alone. MemoryCovDecoder's covariance branch only reads the shared GRU input and never feeds back into the
+    flow, so with the same weights both variants compute the same flow; the plain one skips the covariance GRU unit, the
+    covariance head and the covariance mask / upsampling, and `inference` returns (flow, None)."""
 
     def __init__(self, state_dict: dict[str, Tensor], device, enc_dtype=torch.float32, dec_dtype=torch.float32,
                  decoder_depth: int = 12,
                  corr_fn: Callable[[Tensor, Tensor], Tensor] | None = None,
-                 lookup_fn: Callable[[Tensor, Tensor], Tensor] | None = None):
+                 lookup_fn: Callable[[Tensor, Tensor], Tensor] | None = None,
+                 covariance: bool = True):
         self.device = torch.device(device)
         self.enc_dtype, self.dec_dtype, self.depth = enc_dtype, dec_dtype, decoder_depth
+        self.covariance = bool(covariance)
         # TF32 mode only: the 128-channel transformer MLPs as one fused kernel (MACVO_B200_MLP_TC=0: cuBLAS GEMMs + GELU + add)
         self.mlp_tensor_cores = os.environ.get("MACVO_B200_MLP_TC", "1") != "0"
         self._ops = None
@@ -269,11 +281,12 @@ class FlowFormerCovNet:
 
     # ---- weights -------------------------------------------------------------------------------
     def load_state_dict(self, ckpt: dict[str, Tensor]) -> None:
-        """Accepts the reference checkpoint layout incl. DDP `module.` prefixes (flownet.py:46-53)."""
+        """Accepts the reference checkpoint layout incl. DDP `module.` prefixes (flownet.py:46-53). Keys this variant does
+        not use are ignored (a FlowFormerCov checkpoint loads into the plain network); missing ones raise."""
         ckpt = {(k[7:] if k.startswith("module.") else k): v for k, v in ckpt.items()}
         W: dict[str, Tensor] = {}
         missing = []
-        for key, shape, _ in param_spec():
+        for key, shape, _ in param_spec(self.covariance):
             if key not in ckpt:
                 missing.append(key)
                 continue
@@ -293,7 +306,7 @@ class FlowFormerCovNet:
             raise KeyError(f"checkpoint misses {len(missing)} tensors, e.g. {missing[:3]}")
         self.W = W
         # fused GRU gate filters (z|r share their input)
-        for p in ("memory_decoder.update_block.gru.", "memory_decoder.cov_update.gru."):
+        for p in ("memory_decoder.update_block.gru.",) + ((COV_PREFIX + "gru.",) if self.covariance else ()):
             for o in "12":
                 W[p + f"convzr{o}.weight"] = torch.cat([W[p + f"convz{o}.weight"], W[p + f"convr{o}.weight"]], 0).contiguous(
                     memory_format=torch.channels_last)
@@ -309,7 +322,7 @@ class FlowFormerCovNet:
         W[e + "convp.bias"] = F.pad(W[e + "conv.bias"], (0, 2)).contiguous()
 
     def state_dict(self) -> dict[str, Tensor]:
-        return {k: self.W[k] for k, _, _ in param_spec()}
+        return {k: self.W[k] for k, _, _ in param_spec(self.covariance)}
 
     def _lin(self, x: Tensor, p: str) -> Tensor:
         return F.linear(x, self.W[p + ".weight"], self.W.get(p + ".bias"))
@@ -682,7 +695,7 @@ class FlowFormerCovNet:
 
     def _make_decoder_tc(self, B: int, H: int, W: int, device):
         """Buffers (fp16 padded pixel rows, csrc/rows_layout.cuh) and packed filters of the tensor-core decoder iteration
-        (csrc/conv_tc.cu): motion encoder, value projection, flow head, covariance head."""
+        (csrc/conv_tc.cu): motion encoder, value projection, flow head, covariance head (covariance network only)."""
         from types import SimpleNamespace
         ops, m = self._ops, "memory_decoder."
         e, ub, cu = m + "update_block.encoder.", m + "update_block.", m + "cov_update."
@@ -690,11 +703,11 @@ class FlowFormerCovNet:
         u16 = lambda c: torch.zeros(rows, c, dtype=torch.float16, device=device)
         t = SimpleNamespace(shape=(B, H, W))
         t.tok16, t.c1, t.cp, t.f1, t.mf16 = u16(192), u16(256), u16(256), u16(128), u16(128)
-        t.fh, t.ch1, t.ch2, t.ch3 = u16(256), u16(256), u16(128), u16(64)
+        t.fh = u16(256)
         t.f0 = torch.zeros(P, 128, dtype=torch.float16, device=device)            # im2col rows of the flow (dense)
         t.v16 = torch.zeros(P, 128, dtype=torch.float16, device=device)
         t.mf32 = torch.zeros(P, 128, dtype=torch.float32, device=device)
-        t.d_flow, t.d_cov = (torch.zeros(P, 2, dtype=torch.float32, device=device) for _ in range(2))
+        t.d_flow = torch.zeros(P, 2, dtype=torch.float32, device=device)
         pk = lambda name, cin=None: ops.pack_conv_filter(self.W[name + ".weight"], self.W.get(name + ".bias"), cin, device)
         t.convc1 = pk(e + "convc1p", 192)
         t.convc2, t.convf2, t.conv = pk(e + "convc2"), pk(e + "convf2"), pk(e + "conv")
@@ -702,7 +715,10 @@ class FlowFormerCovNet:
         t.convf1 = ops.pack_conv_filter(wf1.permute(0, 2, 3, 1).reshape(wf1.shape[0], 98, 1, 1), self.W[e + "convf1.bias"], 128, device)
         t.to_v = pk(ub + "aggregator.to_v")
         t.fh1, t.fh2 = pk(ub + "flow_head.conv1"), pk(ub + "flow_head.conv2")
-        t.chw = [pk(cu + f"cov_head.conv{i}") for i in (1, 2, 3, 4)]
+        if self.covariance:
+            t.ch1, t.ch2, t.ch3 = u16(256), u16(128), u16(64)
+            t.d_cov = torch.zeros(P, 2, dtype=torch.float32, device=device)
+            t.chw = [pk(cu + f"cov_head.conv{i}") for i in (1, 2, 3, 4)]
         return t
 
     @staticmethod
@@ -724,15 +740,16 @@ class FlowFormerCovNet:
             return "tf32"
         return "strict"
 
-    def memory_decoder(self, cost_memory: Tensor, context: Tensor, cost_maps: Tensor) -> tuple[Tensor, Tensor]:
+    def memory_decoder(self, cost_memory: Tensor, context: Tensor, cost_maps: Tensor) -> tuple[Tensor, Tensor | None]:
         m, dd = "memory_decoder.", self.dec_dtype
         cost_memory = cost_memory.to(dd)
         B, _, H1, W1 = context.shape
         coords0 = coords_grid(B, H1, W1, context.device, context.dtype)
-        coords1, ccoords1 = coords0.clone(), coords0.clone()
+        coords1 = coords0.clone()
+        ccoords1 = coords0.clone() if self.covariance else None
         ctx = self._conv(context, m + "proj")
         net = ctx[:, :128].tanh().to(dd)
-        cnet = net.clone()
+        cnet = net.clone() if self.covariance else None
         inp = ctx[:, 128:].relu().to(dd)
         mode = self._decoder_mode(ctx)
         # GMA attention, once per frame (gma.py:39-82): softmax over the N x N similarity
@@ -753,23 +770,23 @@ class FlowFormerCovNet:
         value = self._lin(cost_memory, ca + "v")
         refine = {"tf32": self._refine_tf32, "strict": self._refine_strict, "torch": self._refine_torch}[mode]
         coords1, ccoords1, net, cnet = refine(coords0, coords1, ccoords1, net, cnet, inp, attention, key, value, cost_maps)
-        # the reference evaluates both mask heads + upsampling every iteration but (eval mode) returns
-        # only the last one (covhead.py:137-140) -> evaluate once
+        # the reference evaluates the mask heads + upsampling every iteration but (eval mode) returns
+        # only the last one (covhead.py:137-140, decoder.py:197-203) -> evaluate once
         ub, cu = m + "update_block.", m + "cov_update."
         if mode != "torch":     # scale + softmax + unfold + weighted sum + pixel shuffle in one kernel per map
-            up_logits = self._conv(self._conv_relu(net, ub + "mask.0", padding=1), ub + "mask.2")
-            cov_logits = self._conv(self._conv_relu(cnet, cu + "mask.0", padding=1), cu + "mask.2")
-            return (self._ops.convex_upsample(coords1 - coords0, up_logits, 0.25),
-                    self._ops.convex_upsample(ccoords1 - coords0, cov_logits, 0.25))
-        up_mask = _f32(0.25 * self._conv(F.relu(self._conv(net, ub + "mask.0", padding=1)), ub + "mask.2"))
-        cov_mask = _f32(0.25 * self._conv(F.relu(self._conv(cnet, cu + "mask.0", padding=1)), cu + "mask.2"))
-        return self.convex_upsample(coords1 - coords0, up_mask), self.convex_upsample(ccoords1 - coords0, cov_mask)
+            upsample = lambda c1, h, p: self._ops.convex_upsample(
+                c1 - coords0, self._conv(self._conv_relu(h, p + "mask.0", padding=1), p + "mask.2"), 0.25)
+        else:
+            upsample = lambda c1, h, p: self.convex_upsample(
+                c1 - coords0, _f32(0.25 * self._conv(F.relu(self._conv(h, p + "mask.0", padding=1)), p + "mask.2")))
+        flow = upsample(coords1, net, ub)
+        return flow, (upsample(ccoords1, cnet, cu) if self.covariance else None)
 
     def _refine_tf32(self, coords0, coords1, ccoords1, net, cnet, inp, attention, key, value, cost_maps):
         """The whole iteration on our kernels: lookup, token kernel, motion encoder / value projection / heads on the
-        tensor-core convolution kernel (fp16 rows between the layers), both SepConvGRU units on their tensor-core kernel (fp16
-        operands, fp32 state; csrc/gru_conv_tc.cu); the one library call left is the GMA aggregation GEMM over the fp16
-        `attention`."""
+        tensor-core convolution kernel (fp16 rows between the layers), the SepConvGRU units (flow, and covariance when the network
+        has one) on their tensor-core kernel (fp16 operands, fp32 state; csrc/gru_conv_tc.cu); the one library call left is the
+        GMA aggregation GEMM over the fp16 `attention`."""
         m = "memory_decoder."
         ub, cu = m + "update_block.", m + "cov_update."
         ops = self._ops
@@ -780,18 +797,19 @@ class FlowFormerCovNet:
         side2 = self._memo(("side_stream2", dev), lambda: torch.cuda.Stream(dev))
         as_map = lambda t: t.view(B, H1, W1, -1).permute(0, 3, 1, 2)                   # channels_last logical map
 
+        units = (ub, cu) if self.covariance else (ub,)
+
         def make_gru():
             names = [f"conv{g}{o}" for g in ("zr", "q") for o in ("1", "2")]
-            ws = [{n: self.W[pre + "gru." + n + ".weight"] for n in names} for pre in (ub, cu)]
-            bs = [{n: self.W[pre + "gru." + n + ".bias"] for n in names} for pre in (ub, cu)]
+            ws = [{n: self.W[pre + "gru." + n + ".weight"] for n in names} for pre in units]
+            bs = [{n: self.W[pre + "gru." + n + ".bias"] for n in names} for pre in units]
             return ops.SepConvGruTC(ws, bs, B, H1, W1, dev)
         gru = self._memo(("gru_tc", B, H1, W1, dev), make_gru)
         t = self._memo(("decoder_tc", B, H1, W1, dev), lambda: self._make_decoder_tc(B, H1, W1, dev))
         gru.set_context(inp.permute(0, 2, 3, 1).reshape(P, 128).contiguous())
         net_rows = net.permute(0, 2, 3, 1).reshape(P, 128).contiguous()
-        gru.set_state(0, net_rows)
-        gru.set_state(1, net_rows)
-        net_d, cnet_d = gru.h
+        for u in range(len(units)):
+            gru.set_state(u, net_rows)
         token_blob = self._memo(("token_blob", dev), lambda: ops.decoder_token_blob(self.W, m))
         key, value = key.contiguous(), value.contiguous()
         gamma = self.W[ub + "aggregator.gamma"]
@@ -820,24 +838,27 @@ class FlowFormerCovNet:
             # one launch chain per GRU unit on two streams; the covariance unit's chain ends in `unit1_done`, which only the
             # covariance head waits for
             unit1_done = gru.step(t.mf32, agg.view(P, 128), gamma)
-            # The covariance head (4 chained convolutions, covhead.py:20-58) feeds only the covariance coordinates: it runs on
-            # its own stream and is joined right before the NEXT iteration's GRU update, so it overlaps the next lookup / token
-            # kernel / motion encoder instead of extending this iteration (they depend on the flow head only).
-            with torch.cuda.stream(side2):
-                side2.wait_event(unit1_done)
-                ops.conv_tc(gru.h_rows[0][1], t.chw[0][0], t.chw[0][1], 256, 3, True, shp, out16=t.ch1)
-                ops.conv_tc(t.ch1, t.chw[1][0], t.chw[1][1], 128, 3, False, shp, out16=t.ch2)
-                ops.conv_tc(t.ch2, t.chw[2][0], t.chw[2][1], 64, 3, True, shp, out16=t.ch3)
-                ops.conv_tc(t.ch3, t.chw[3][0], t.chw[3][1], 2, 3, False, shp, add_to_map=ccoords1)   # ccoords1 += delta (in the epilogue)
-                cov_done = torch.cuda.Event()
-                cov_done.record(side2)
+            if self.covariance:
+                # The covariance head (4 chained convolutions, covhead.py:20-58) feeds only the covariance coordinates: it runs
+                # on its own stream and is joined right before the NEXT iteration's GRU update, so it overlaps the next lookup /
+                # token kernel / motion encoder instead of extending this iteration (they depend on the flow head only).
+                with torch.cuda.stream(side2):
+                    side2.wait_event(unit1_done)
+                    ops.conv_tc(gru.h_rows[0][1], t.chw[0][0], t.chw[0][1], 256, 3, True, shp, out16=t.ch1)
+                    ops.conv_tc(t.ch1, t.chw[1][0], t.chw[1][1], 128, 3, False, shp, out16=t.ch2)
+                    ops.conv_tc(t.ch2, t.chw[2][0], t.chw[2][1], 64, 3, True, shp, out16=t.ch3)
+                    ops.conv_tc(t.ch3, t.chw[3][0], t.chw[3][1], 2, 3, False, shp, add_to_map=ccoords1)   # ccoords1 += delta
+                    cov_done = torch.cuda.Event()
+                    cov_done.record(side2)
             ops.conv_tc(gru.h_rows[0][0], t.fh1[0], t.fh1[1], 256, 3, True, shp, out16=t.fh)
             ops.conv_tc(t.fh, t.fh2[0], t.fh2[1], 2, 3, False, shp, add_to_map=coords1)               # coords1 += delta_flow
-            if self.taps is not None:
+            if self.taps is not None and cov_done is not None:
                 main.wait_event(cov_done)
-            net, cnet = as_map(net_d), as_map(cnet_d)
+            net = as_map(gru.h[0])
             self._tap("flow_iter", coords1 - coords0)
-            self._tap("cov_iter", ccoords1 - coords0)
+            if self.covariance:
+                cnet = as_map(gru.h[1])
+                self._tap("cov_iter", ccoords1 - coords0)
         if cov_done is not None:
             torch.cuda.current_stream().wait_event(cov_done)
         return coords1, ccoords1, net, cnet
@@ -856,13 +877,14 @@ class FlowFormerCovNet:
         inp_rows = inp.permute(0, 2, 3, 1).reshape(P, 128).contiguous()
         net_rows = net.permute(0, 2, 3, 1).reshape(P, 128).contiguous()
         # recurrent state in NHWC [h | x] buffers (csrc/decoder_fused.cu): x = [inp | mf | mf + gamma*agg]
-        bufs = [torch.empty(P, 512, dtype=dd, device=dev) for _ in range(4)]   # hx, rhx (flow) / hx, rhx (cov)
+        bufs = [torch.empty(P, 512, dtype=dd, device=dev) for _ in range(4 if self.covariance else 2)]   # hx, rhx (flow) / (cov)
         for bf in bufs:
             bf[:, 128:256] = inp_rows
         bufs[0][:, :128] = net_rows
-        bufs[2][:, :128] = bufs[0][:, :128]
-        zbuf, zbuf2 = torch.empty(P, 128, dtype=dd, device=dev), torch.empty(P, 128, dtype=dd, device=dev)
-        net_d, cnet_d = torch.empty(P, 128, dtype=dd, device=dev), torch.empty(P, 128, dtype=dd, device=dev)
+        zbuf, net_d = torch.empty(P, 128, dtype=dd, device=dev), torch.empty(P, 128, dtype=dd, device=dev)
+        if self.covariance:
+            bufs[2][:, :128] = bufs[0][:, :128]
+            zbuf2, cnet_d = torch.empty(P, 128, dtype=dd, device=dev), torch.empty(P, 128, dtype=dd, device=dev)
         token_blob = self._memo(("token_blob", dev), lambda: ops.decoder_token_blob(self.W, m))
         key, value = key.contiguous(), value.contiguous()
         gamma = self.W[ub + "aggregator.gamma"]
@@ -898,26 +920,28 @@ class FlowFormerCovNet:
             # at 60x80 each conv fills about two thirds of the 132 SMs, so the two run on forked streams (fork/join is
             # captured into the CUDA graph as parallel branches)
             ops.gru_input(mf.permute(0, 2, 3, 1), agg, gamma, bufs)
-            main = torch.cuda.current_stream()
-            fork = torch.cuda.Event()
-            fork.record(main)
-            with torch.cuda.stream(side):
-                side.wait_event(fork)
-                self._gru_native(bufs[2], bufs[3], zbuf2, cu + "gru.", cnet_d, (B, H1, W1))
-                cnet = as_map(cnet_d)
-                h = cu + "cov_head."
-                t = self._conv(self._conv_relu(cnet, h + "conv1", padding=1), h + "conv2", padding=1)
-                d_cov = self._conv(self._conv_relu(t, h + "conv3", padding=1), h + "conv4", padding=1)
-                join = torch.cuda.Event()
-                join.record(side)
+            if self.covariance:
+                main = torch.cuda.current_stream()
+                fork = torch.cuda.Event()
+                fork.record(main)
+                with torch.cuda.stream(side):
+                    side.wait_event(fork)
+                    self._gru_native(bufs[2], bufs[3], zbuf2, cu + "gru.", cnet_d, (B, H1, W1))
+                    cnet = as_map(cnet_d)
+                    h = cu + "cov_head."
+                    t = self._conv(self._conv_relu(cnet, h + "conv1", padding=1), h + "conv2", padding=1)
+                    d_cov = self._conv(self._conv_relu(t, h + "conv3", padding=1), h + "conv4", padding=1)
+                    join = torch.cuda.Event()
+                    join.record(side)
             self._gru_native(bufs[0], bufs[1], zbuf, ub + "gru.", net_d, (B, H1, W1))
             net = as_map(net_d)
             d_flow = self._conv(self._conv_relu(net, ub + "flow_head.conv1", padding=1), ub + "flow_head.conv2", padding=1)
-            main.wait_event(join)
             coords1 = coords1 + d_flow
-            ccoords1 = ccoords1 + d_cov
             self._tap("flow_iter", coords1 - coords0)
-            self._tap("cov_iter", ccoords1 - coords0)
+            if self.covariance:
+                main.wait_event(join)
+                ccoords1 = ccoords1 + d_cov
+                self._tap("cov_iter", ccoords1 - coords0)
         return coords1, ccoords1, net, cnet
 
     def _refine_torch(self, coords0, coords1, ccoords1, net, cnet, inp, attention, key, value, cost_maps):
@@ -953,15 +977,16 @@ class FlowFormerCovNet:
             agg = torch.matmul(attention, v)                                    # (B, N, 128) = pixels-major
             inp_cat = torch.cat([inp, mf, mf + gamma * agg.transpose(1, 2).reshape(B, 128, H1, W1)], dim=1)
             net = self._gru(net, inp_cat, ub + "gru.")
-            cnet = self._gru(cnet, inp_cat, cu + "gru.")
             d_flow = self._conv(self._conv_relu(net, ub + "flow_head.conv1", padding=1), ub + "flow_head.conv2", padding=1)
-            h = cu + "cov_head."
-            t = self._conv(self._conv_relu(cnet, h + "conv1", padding=1), h + "conv2", padding=1)
-            d_cov = self._conv(self._conv_relu(t, h + "conv3", padding=1), h + "conv4", padding=1)
             coords1 = coords1 + _f32(d_flow)
-            ccoords1 = ccoords1 + _f32(d_cov)
             self._tap("flow_iter", coords1 - coords0)
-            self._tap("cov_iter", ccoords1 - coords0)
+            if self.covariance:
+                cnet = self._gru(cnet, inp_cat, cu + "gru.")
+                h = cu + "cov_head."
+                t = self._conv(self._conv_relu(cnet, h + "conv1", padding=1), h + "conv2", padding=1)
+                d_cov = self._conv(self._conv_relu(t, h + "conv3", padding=1), h + "conv4", padding=1)
+                ccoords1 = ccoords1 + _f32(d_cov)
+                self._tap("cov_iter", ccoords1 - coords0)
         return coords1, ccoords1, net, cnet
 
     # ---- top level (flownet.py:18-44) -----------------------------------------------------------
@@ -999,16 +1024,16 @@ class FlowFormerCovNet:
             self._ctx_join = None
 
     @torch.inference_mode()
-    def inference(self, image1: Tensor, image2: Tensor, shared: tuple[int, int] | None = None) -> tuple[Tensor, Tensor]:
-        """(B,3,H,W) x2 in [0,1] -> flow (B,2,H,W), cov = exp(2 log sigma) (B,2,H,W); shared = (i, j) promises that image2[j] is
-        image1[i] (it is then encoded once, see `memory_encoder`)."""
+    def inference(self, image1: Tensor, image2: Tensor, shared: tuple[int, int] | None = None) -> tuple[Tensor, Tensor | None]:
+        """(B,3,H,W) x2 in [0,1] -> flow (B,2,H,W), cov = exp(2 log sigma) (B,2,H,W), or None for the plain network;
+        shared = (i, j) promises that image2[j] is image1[i] (it is then encoded once, see `memory_encoder`)."""
         H, W = image1.shape[-2:]
         ph, pw = (-H) % 8, (-W) % 8
         pad = [pw // 2, pw - pw // 2, ph // 2, ph - ph // 2]       # InputPadder 'sintel' (core/utils.py:4-24)
         if ph or pw:
             image1, image2 = F.pad(image1, pad, mode="replicate"), F.pad(image2, pad, mode="replicate")
         flow, logsig = self.forward(image1, image2, shared)
-        if ph or pw:
-            flow = flow[..., pad[2]:flow.shape[-2] - pad[3], pad[0]:flow.shape[-1] - pad[1]]
-            logsig = logsig[..., pad[2]:logsig.shape[-2] - pad[3], pad[0]:logsig.shape[-1] - pad[1]]
-        return flow, torch.exp(logsig * 2)
+        unpad = (lambda t: t[..., pad[2]:t.shape[-2] - pad[3], pad[0]:t.shape[-1] - pad[1]]) if ph or pw else (lambda t: t)
+        if logsig is None:
+            return unpad(flow), None
+        return unpad(flow), torch.exp(unpad(logsig) * 2)

@@ -274,13 +274,26 @@ class ScoreBuffers:
                        self.cand_vals2.data_ptr() if dcov0 is not None else None)
 
 
-def dense_postproc(est_flow: Tensor, est_cov: Tensor, bl_fx: float, enforce_positive_disparity: bool = False,
+def dense_postproc(est_flow: Tensor, est_cov: Tensor | None, bl_fx: float, enforce_positive_disparity: bool = False,
                    score: ScoreBuffers | None = None) -> dict:
     """One `estimate_pair` of dense maps (Frontend.py:184-200, 291-299) + optional fused keypoint scoring.
 
-    est_flow / est_cov: (2,2,H,W) fp32. bl_fx = baseline*fx as a python float (double), like the reference."""
+    est_flow / est_cov: (2,2,H,W) fp32. bl_fx = baseline*fx as a python float (double), like the reference.
+    est_cov None (a frontend without covariance, FlowFormerDepth / FlowFormerMatcher): est_flow (1|2,2,H,W); depth and
+    disparity of slot 0, the flow of slot 1 (None for one slot); every covariance / mask output is None."""
     lib = load_library()
     fl = _dev(est_flow, torch.float32, "dense_postproc est_flow")
+    if est_cov is None:
+        if enforce_positive_disparity or score is not None or fl.dim() != 4 or fl.shape[0] not in (1, 2) or fl.shape[1] != 2:
+            raise MacvoB200Error("dense_postproc without est_cov: expects est_flow (1|2,2,H,W) and no mask or scoring")
+        H, W = fl.shape[-2:]
+        depth = torch.empty((1, 1, H, W), dtype=torch.float32, device=fl.device)
+        disparity = torch.empty_like(depth)
+        _check(lib.macvo_dense_postproc(fl.data_ptr(), None, H, W, float(bl_fx), float(bl_fx) ** 2, depth.data_ptr(),
+                                        disparity.data_ptr(), None, None, None, None, _stream()), "macvo_dense_postproc")
+        LAUNCHES[0] += 1
+        return {"depth": depth, "disparity": disparity, "depth_cov": None, "disparity_uncertainty": None, "depth_mask": None,
+                "flow": fl[1:2] if fl.shape[0] == 2 else None, "flow_cov": None}
     cv = _dev(est_cov, torch.float32, "dense_postproc est_cov")
     assert fl.shape[:2] == (2, 2) and cv.shape == fl.shape
     H, W = fl.shape[-2:]
@@ -682,8 +695,8 @@ def cov_modify(cov: Tensor, ops: list[str] | tuple[str, ...]) -> Tensor:
     return cov
 
 
-def observe_pack(buf: ObservationBuffers, kp0_uv: Tensor, flow: Tensor, match_cov: Tensor, depth0: Tensor, depth1: Tensor,
-                 disparity1: Tensor, disp_unc1: Tensor, edge_width: int, intr0, intr1, prev_pose: Tensor, next_pose: Tensor,
+def observe_pack(buf: ObservationBuffers, kp0_uv: Tensor, flow: Tensor, match_cov: Tensor | None, depth0: Tensor, depth1: Tensor,
+                 disparity1: Tensor, disp_unc1: Tensor | None, edge_width: int, intr0, intr1, prev_pose: Tensor, next_pose: Tensor,
                  kernel_size: int = 31, min_flow_cov: float = 0.25, min_depth_cov: float = 0.05,
                  match_cov_default: float = 0.25, ext: dict | None = None) -> None:
     """Odometry/MACVO.py:198-283 for the two-frame graph as two launches (csrc/observe.cu); everything stays on the device.
@@ -691,15 +704,21 @@ def observe_pack(buf: ObservationBuffers, kp0_uv: Tensor, flow: Tensor, match_co
     ext (None: CovarianceSanityFilter only) = macvo_observe_ext_t as a dict: depth_cov0 / depth_cov1 ((1,1,H,W) fp32 CUDA
     or None), simple_depth (bool), min_depth / max_depth (floats, rounded to fp32 like the reference's comparisons),
     front_of_cam (bool), icp (bool: pack the "icp" graph's columns; needs an extended buffer), cov_model ("match" or
-    "identity", the NoCovariance model) and cov_ops (modifier names of COV_OPS, innermost first)."""
+    "identity", the NoCovariance model) and cov_ops (modifier names of COV_OPS, innermost first).
+
+    match_cov and disp_unc1 both None: a frontend without covariance maps (pixel2_uv_cov / pixel2_disp_cov hold -1, kp1's
+    MatchCovariance uses match_cov_default unclamped; include/macvo_b200.h)."""
     lib = load_library()
     kp = _dev(kp0_uv, torch.int64, "observe_pack kp0_uv")
     k = kp.shape[0]
     fl = _dev(flow, torch.float32, "observe_pack flow")
-    mc = _dev(match_cov, torch.float32, "observe_pack match_cov")
-    maps = [_dev(t, torch.float32, "observe_pack map") for t in (depth0, depth1, disparity1, disp_unc1)]
+    if (match_cov is None) != (disp_unc1 is None):
+        raise MacvoB200Error("observe_pack: match_cov and disp_unc1 are None together (no frontend covariance) or not at all")
+    mc = None if match_cov is None else _dev(match_cov, torch.float32, "observe_pack match_cov")
+    maps = [None if t is None else _dev(t, torch.float32, "observe_pack map") for t in (depth0, depth1, disparity1, disp_unc1)]
     H, W = fl.shape[-2:]
-    if fl.numel() != 2 * H * W or mc.numel() != 3 * H * W or any(m.numel() != H * W for m in maps):
+    if (fl.numel() != 2 * H * W or (mc is not None and mc.numel() != 3 * H * W)
+            or any(m is not None and m.numel() != H * W for m in maps)):
         raise MacvoB200Error("observe_pack: expects flow (1,2,H,W), match_cov (1,3,H,W) and (1,1,H,W) maps")
     if k > buf.capacity:
         raise MacvoB200Error(f"observe_pack: {k} keypoints exceed the buffer capacity {buf.capacity}")
@@ -728,8 +747,8 @@ def observe_pack(buf: ObservationBuffers, kp0_uv: Tensor, flow: Tensor, match_co
         ops_ = tuple(ext.get("cov_ops", ()))
         xs.cov_model, xs.cov_ops, xs.n_cov_ops = COV_MODELS[model], _cov_ops(ops_, "observe_pack"), len(ops_)
     buf.status.zero_()
-    rc = lib.macvo_observe_pack(kp.data_ptr() if k else None, k, buf.capacity, fl.data_ptr(), mc.data_ptr(),
-                                *(m.data_ptr() for m in maps), H, W, int(edge_width), C.cast(i0, C.c_void_p),
+    rc = lib.macvo_observe_pack(kp.data_ptr() if k else None, k, buf.capacity, fl.data_ptr(), None if mc is None else mc.data_ptr(),
+                                *(None if m is None else m.data_ptr() for m in maps), H, W, int(edge_width), C.cast(i0, C.c_void_p),
                                 C.cast(i1, C.c_void_p), int(kernel_size), float(min_flow_cov), float(min_depth_cov),
                                 float(match_cov_default), pp.data_ptr(), next_pose.data_ptr(), buf.packed.data_ptr(),
                                 buf.n_obs.data_ptr(), buf.status.data_ptr(), buf.ws.data_ptr(), buf.ws_bytes, _stream(),
@@ -1096,30 +1115,32 @@ def pack_rows(src: Tensor, dst: Tensor, offset: int, shape: tuple[int, int, int]
 
 
 class SepConvGruTC:
-    """The decoder's two SepConvGRU units (gru.py:22-43; flow + covariance, covhead.py:95-131) on the tensor-core path
-    (csrc/gru_conv_tc.cu): fp32 recurrent state `h[u]` (pixels, 128) in dense pixel order, fp16 padded operand rows for the two
-    passes, one `step` = pack the motion features + one 4-launch chain per unit.
+    """The decoder's SepConvGRU units (gru.py:22-43; flow, and covariance for FlowFormerCov, covhead.py:95-131) on the
+    tensor-core path (csrc/gru_conv_tc.cu): fp32 recurrent state `h[u]` (pixels, 128) in dense pixel order, fp16 padded operand
+    rows for the two passes, one `step` = pack the motion features + one 4-launch chain per unit.
 
     weights[u]: {"convzr1": (256,512,1,5), "convq1": (128,512,1,5), "convzr2": (256,512,5,1), "convq2": (128,512,5,1)} fp32
-    filters with the z | r filters concatenated, biases[u]: the matching (N,) vectors; u = 0 flow, 1 covariance."""
+    filters with the z | r filters concatenated, biases[u]: the matching (N,) vectors; u = 0 flow, 1 covariance (one unit:
+    the plain FlowFormer's flow unit alone)."""
 
-    UNITS = 2
+    LAUNCHES_PER_UNIT = 4
 
     def __init__(self, weights: list[dict], biases: list[dict], batch: int, height: int, width: int, device):
         lib = load_library()
         self.shape, self.device = (int(batch), int(height), int(width)), device
-        if len(weights) != self.UNITS or len(biases) != self.UNITS:
-            raise MacvoB200Error("SepConvGruTC: expects the decoder's two units (flow, covariance)")
+        self.units = len(weights)
+        if self.units not in (1, 2) or len(biases) != self.units:
+            raise MacvoB200Error("SepConvGruTC: expects the decoder's flow unit, optionally followed by its covariance unit")
         P = batch * height * width
         rows = [int(lib.macvo_gru_tc_operand_rows(batch, height, width, o)) for o in (0, 1)]
         f16 = dict(dtype=torch.float16, device=device)
         self.x = [torch.zeros(r, 3 * GRU_HID, **f16) for r in rows]
-        self.h_rows = [[torch.zeros(r, GRU_HID, **f16) for _ in range(self.UNITS)] for r in rows]     # [pass][unit]
-        self.rh_rows = [[torch.zeros(r, GRU_HID, **f16) for _ in range(self.UNITS)] for r in rows]
-        self.h = [torch.zeros(P, GRU_HID, dtype=torch.float32, device=device) for _ in range(self.UNITS)]
-        self.z = [torch.zeros(P, GRU_HID, dtype=torch.float32, device=device) for _ in range(self.UNITS)]
+        self.h_rows = [[torch.zeros(r, GRU_HID, **f16) for _ in range(self.units)] for r in rows]     # [pass][unit]
+        self.rh_rows = [[torch.zeros(r, GRU_HID, **f16) for _ in range(self.units)] for r in rows]
+        self.h = [torch.zeros(P, GRU_HID, dtype=torch.float32, device=device) for _ in range(self.units)]
+        self.z = [torch.zeros(P, GRU_HID, dtype=torch.float32, device=device) for _ in range(self.units)]
         self.w, self.b = {}, {}
-        for u in range(self.UNITS):
+        for u in range(self.units):
             for o in (0, 1):
                 for st, name in ((0, f"convzr{o + 1}"), (1, f"convq{o + 1}")):
                     w = weights[u][name].detach().to(device=device, dtype=torch.float32)
@@ -1132,8 +1153,8 @@ class SepConvGruTC:
         self._stage_args = {(u, o, st): ((self.h_rows[o] if st == 0 else self.rh_rows[o])[u].data_ptr(), self.x[o].data_ptr(),
                                          self.w[u, o, st].data_ptr(), self.b[u, o, st].data_ptr(), self.h[u].data_ptr(),
                                          self.z[u].data_ptr(), (self.rh_rows[o] if st == 0 else self.h_rows[1 - o])[u].data_ptr())
-                            for u in range(self.UNITS) for o in (0, 1) for st in (0, 1)}
-        self._side = torch.cuda.Stream(device)
+                            for u in range(self.units) for o in (0, 1) for st in (0, 1)}
+        self._side = torch.cuda.Stream(device) if self.units == 2 else None
 
     def _pack(self, src: Tensor, dst: Tensor, offset: int, vertical: int) -> None:
         B, H, W = self.shape
@@ -1153,12 +1174,13 @@ class SepConvGruTC:
         self.h[unit].copy_(_dense(h_rows, GRU_HID, "SepConvGruTC state").view(-1, GRU_HID))
         self._pack(self.h[unit], self.h_rows[0][unit], 0, 0)
 
-    def step(self, mf: Tensor, agg: Tensor, gamma: Tensor) -> torch.cuda.Event:
-        """one SepConvGRU update of both units with x = [inp | mf | mf + gamma * agg]; new state in `self.h[u]`.
+    def step(self, mf: Tensor, agg: Tensor, gamma: Tensor) -> torch.cuda.Event | None:
+        """one SepConvGRU update of every unit with x = [inp | mf | mf + gamma * agg]; new state in `self.h[u]`.
         One 4-launch chain per unit: with 84 CTA tiles per unit (640x480: two 60x80 maps) a launch covering both units would be
         168 CTAs = two waves on 132 SMs per stage, two independent chains of 84-CTA launches keep the SMs filled across the stage
         boundaries. Unit 0's chain runs on the current stream, unit 1's on a side stream; the returned event marks the end of
-        unit 1's chain, and whatever reads unit 1's state must make its stream wait on it."""
+        unit 1's chain, and whatever reads unit 1's state must make its stream wait on it. With one unit there is no side
+        stream and no event (None)."""
         B, H, W = self.shape
         lib = load_library()
         mf, agg = _dense(mf, GRU_HID, "SepConvGruTC mf"), _dense(agg, GRU_HID, "SepConvGruTC agg")
@@ -1168,14 +1190,16 @@ class SepConvGruTC:
         _check(lib.macvo_gru_tc_pack_motion(mf.data_ptr(), agg.data_ptr(), _dev(gamma, torch.float32, "gamma").data_ptr(),
                                             self.x[0].data_ptr(), self.x[1].data_ptr(), B, H, W, main.cuda_stream),
                "macvo_gru_tc_pack_motion")
-        fork = torch.cuda.Event()
-        fork.record(main)
-        self._side.wait_event(fork)
-        self._chain(1, self._side)
-        unit1_done = torch.cuda.Event()
-        unit1_done.record(self._side)
+        unit1_done = None
+        if self.units == 2:
+            fork = torch.cuda.Event()
+            fork.record(main)
+            self._side.wait_event(fork)
+            self._chain(1, self._side)
+            unit1_done = torch.cuda.Event()
+            unit1_done.record(self._side)
         self._chain(0, main)
-        LAUNCHES[0] += 9
+        LAUNCHES[0] += 1 + self.LAUNCHES_PER_UNIT * self.units
         return unit1_done
 
     def _chain(self, unit: int, stream: torch.cuda.Stream) -> None:

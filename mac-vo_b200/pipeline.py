@@ -118,16 +118,19 @@ class TwoFrameOdometry:
         kp0_uv, kp1_uv = kp0_uv[inb], kp1_uv[inb]
         num_kp = kp0_uv.size(0)
 
+        # a frontend without covariance maps (B200_FlowFormerFrontend) gives None here, like MACVO.py:212-232
+        squeeze = lambda t: None if t is None else t.squeeze(0)
         kp0_d = fe.retrieve_pixels(kp0_uv, depth0.depth).squeeze(0)
-        kp0_sigma_dd = fe.retrieve_pixels(kp0_uv, depth0.cov).squeeze(0)
+        kp0_sigma_dd = squeeze(fe.retrieve_pixels(kp0_uv, depth0.cov))
         kp1_disparity = fe.retrieve_pixels(kp1_uv, depth1.disparity)
         kp1_sigma_disparity = fe.retrieve_pixels(kp1_uv, depth1.disparity_uncertainty)
-        kp1_sigma_dd = fe.retrieve_pixels(kp1_uv, depth1.cov).squeeze(0)
+        kp1_sigma_dd = squeeze(fe.retrieve_pixels(kp1_uv, depth1.cov))
 
         dev = kp0_uv.device
         kp0_sigma_uv = torch.ones((num_kp, 3), device=dev) * self.match_cov_default
         kp0_sigma_uv[..., 2] = 0.
-        kp1_sigma_uv = fe.retrieve_pixels(kp0_uv, match01.cov).T.contiguous()
+        kp1_sigma_uv = fe.retrieve_pixels(kp0_uv, match01.cov)
+        kp1_sigma_uv = None if kp1_sigma_uv is None else kp1_sigma_uv.T.contiguous()
 
         K = frame0.frame_K.to(dev)
         fx, fy, cx, cy = K[0, 0], K[1, 1], K[0, 2], K[1, 2]
@@ -158,6 +161,11 @@ class TwoFrameOdometry:
         self.poses.append(est_pose)
         out = None
         if num_obs >= self.min_num_point:
+            # MatchObs' -1 placeholders of the missing covariance columns (MACVO.py:250-264)
+            if kp1_sigma_uv is None:
+                kp1_sigma_uv = torch.full((num_kp, 3), -1.0, device=dev)
+            if kp1_sigma_disparity is None:
+                kp1_sigma_disparity = torch.full((1, num_kp), -1.0, device=dev)
             inp = PGOInput(pos_Tw=pos_Tw, kp2_uv=kp1_uv[keep].float(), kp2_disp=kp1_disparity.T[keep],
                            uv_cov=kp1_sigma_uv[keep], disp_cov=kp1_sigma_disparity.T[keep], K=frame1.frame_K,
                            baseline=frame1.frame_baseline, init_pose=est_pose)
@@ -175,7 +183,7 @@ class TwoFrameOdometry:
             map0_uv = self.map_selector.select_point(frame0, 2000, depth0, depth1, match01)
             n_map = map0_uv.size(0)
             if n_map:
-                map0_sigma_dd = fe.retrieve_pixels(map0_uv, depth0.cov).squeeze(0)
+                map0_sigma_dd = squeeze(fe.retrieve_pixels(map0_uv, depth0.cov))
                 map0_sigma_uv = torch.ones((n_map, 3), device=map0_uv.device) * self.match_cov_default
                 map0_sigma_uv[..., 2] = 0.
                 self.cov_model.estimate(frame0, map0_uv, depth0, map0_sigma_dd, map0_sigma_uv)
@@ -222,7 +230,11 @@ class FusedTwoFrameOdometry:
     The ablation back ends: `kp_selector` may be a B200_RandomSelector, whose keypoints are drawn on the device with no
     candidate count, so that with mapping off a frame has NO host synchronisation (`host_waits` records each frame's
     count). `cov_model` may be B200_NoCovariance or B200_Modifier_Diagonalize / _Normalize around a B200 model
-    (`plugins.cov_spec`): observe_pack applies the model, and the mapping branch gets the same covariances."""
+    (`plugins.cov_spec`): observe_pack applies the model, and the mapping branch gets the same covariances. With
+    B200_NoCovariance the chain may leave out B200_CovarianceSanityFilter (`plugins.check_sanity_chain`).
+
+    A frontend without covariance maps (B200_FlowFormerFrontend, the Vanilla ablation) hands observe_pack NULL maps: the
+    packed pixel2_uv_cov / pixel2_disp_cov columns hold MatchObs' -1 placeholder."""
 
     def __init__(self, frontend, kp_selector, cov_model, optimizer, num_point: int = 200, edgewidth: int = 32,
                  match_cov_default: float = 0.25, mapping: bool = True, map_selector=None, min_num_point: int = 10,
@@ -244,11 +256,12 @@ class FusedTwoFrameOdometry:
         self.num_point, self.edgewidth, self.match_cov_default = num_point, edgewidth, match_cov_default
         self.mapping, self.min_num_point, self.num_map_point = mapping and map_selector is not None, min_num_point, num_map_point
         self.keep_debug = keep_debug
-        self.device = kp_selector.device
-        from .plugins import B200_RandomSelector, cov_spec
-        self.random_kp = isinstance(kp_selector, B200_RandomSelector)   # drawn on the device: no candidate count to wait for
+        from .plugins import B200_RandomSelector, check_sanity_chain, cov_spec
         _, self.cov_ops, params = cov_spec(cov_model)
         self.cov_identity = params is None
+        check_sanity_chain(outlier_filter, covariance_finite=self.cov_identity)
+        self.device = kp_selector.device
+        self.random_kp = isinstance(kp_selector, B200_RandomSelector)   # drawn on the device: no candidate count to wait for
         # B200_NoCovariance has no kernel parameters: observe_pack reads none of them then, and kernel_size 1 reduces the
         # mapping branch's covariance kernel to the point gather at the centre pixel
         self.cov_args = params or dict(kernel_size=1, min_flow_cov=0.25, min_depth_cov=0.05)
@@ -286,7 +299,8 @@ class FusedTwoFrameOdometry:
             from .plugins import observe_ext
             if self.outlier_filter is not None:
                 self.outlier_filter.set_meta(frame0)
-            self.ext = dict(observe_ext(self.outlier_filter) or {}, icp=self.graph_type == "icp", **self.cov_ext)
+            self.ext = dict(observe_ext(self.outlier_filter, covariance_finite=self.cov_identity) or {},
+                            icp=self.graph_type == "icp", **self.cov_ext)
 
     @staticmethod
     def _intr(frame) -> tuple[float, float, float, float]:

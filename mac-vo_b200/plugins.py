@@ -1,6 +1,8 @@
 """B200 plugin classes for MAC-VO's `Module` interfaces (the drop-in boundary, SURVEY.md §8b).
 
     B200_FlowFormerCovFrontend       IFrontend          replaces CUDAGraph_FlowFormerCovFrontend (Frontend.py:264-353)
+    B200_FlowFormerFrontend          IFrontend          replaces FrontendCompose(FlowFormerDepth, FlowFormerMatcher)
+                                                        (Frontend.py:131-155, StereoDepth.py:99-135, Matching.py:120-154)
     B200_CovAwareSelector_NoDepth    IKeypointSelector  replaces CovAwareSelector_NoDepth (KeypointSelector.py:349-407)
     B200_CovAwareSelector            IKeypointSelector  replaces CovAwareSelector (KeypointSelector.py:250-347)
     B200_MappingPointSelector        IKeypointSelector  replaces MappingPointSelector (KeypointSelector.py:78-100)
@@ -73,81 +75,29 @@ def _require_cuda(device: str, who: str) -> torch.device:
 # ================================================================================================
 # Frontend
 # ================================================================================================
-class B200_FlowFormerCovFrontend(IFrontend):
-    """FlowFormerCov stereo + flow frontend: correlation volume and window lookup on sm_90a kernels,
-    dense post-processing + keypoint scoring fused into one pass, the whole `estimate_pair` replayed as a
-    CUDA graph (like CUDAGraph_FlowFormerCovFrontend, Frontend.py:301-353).
+def _load_weights(w, covariance: bool) -> dict:
+    """checkpoint path, or "synthetic[:seed]" for the deterministic stand-in"""
+    if isinstance(w, str) and w.startswith("synthetic"):
+        return synthetic_state_dict(int(w.split(":")[1]) if ":" in w else 0, covariance=covariance)
+    return torch.load(w, map_location="cpu", weights_only=True)
 
-    config: weight (checkpoint path, or "synthetic[:seed]" for the deterministic stand-in), device,
-    enc_dtype / dec_dtype in {fp32, fp16, bf16}, decoder_depth, enforce_positive_disparity,
-    cuda_graph (bool), score_kernel_size (odd int; NMS window of the fused keypoint scoring, 7 in the
-    reference configs)."""
+
+class _B200_GraphedPairFrontend(IFrontend):
+    """What both FlowFormer frontends share: `estimate_pair` as ONE B = 2 network pass, [t2.L, t1.L] against [t2.R, t2.L]
+    (Frontend.py:284-285) with t2.L encoded once, plus the dense post-processing, replayed as a CUDA graph after the first
+    call (like CUDAGraph_FlowFormerCovFrontend, Frontend.py:301-353). Subclasses give `_run` (device images -> the
+    post-processed dict of `ops.dense_postproc`) and `_outputs` (that dict -> the interface's output pair)."""
 
     def __init__(self, config: SimpleNamespace):
         super().__init__(config)
-        self.device = _require_cuda(config.device, "B200_FlowFormerCovFrontend")
-        w = config.weight
-        if isinstance(w, str) and w.startswith("synthetic"):
-            sd = synthetic_state_dict(int(w.split(":")[1]) if ":" in w else 0)
-        else:
-            sd = torch.load(w, map_location="cpu", weights_only=True)
-        enc, dec = _DTYPES[config.enc_dtype], _DTYPES[config.dec_dtype]
-        # MACVO_Fast (enc fp16 / dec bf16, Config/Experiment/MACVO/MACVO_Fast.yaml:8-9) exists because half-precision tensor
-        # cores are the fast path on the GPUs MAC-VO targets. The TF32 pipeline of this class (own kernels + TF32
-        # cuDNN / cuBLAS) is ~4x closer to exact arithmetic than the
-        # reference's own fp16 / bf16 run (flow 9e-4 vs 3.3e-3 of its scale, tests/test_gpu_pipeline.py::test_fast_config_*),
-        # so half-precision configs are served by it unless `half_precision: native` asks for the literal dtypes.
-        self.half_precision = getattr(config, "half_precision", "tf32")
-        if self.half_precision == "tf32":
-            enc = dec = torch.float32
-        self.net = FlowFormerCovNet(sd, self.device, enc, dec, decoder_depth=config.decoder_depth)
-        # the reference frontend enables TF32 tensor cores for the dense layers (Frontend.py:275-277)
-        torch.backends.cuda.matmul.allow_tf32 = True
-        torch.backends.cudnn.allow_tf32 = True
-        torch.set_float32_matmul_precision("medium")
         self._graph = None
         self._static: dict = {}
-        self._score: ops.ScoreBuffers | None = None
 
-    @property
-    def provide_cov(self) -> tuple[bool, bool]:
-        return True, True
-
-    # ---- (a7) + fused (a8) scoring ---------------------------------------------------------------
-    def _postprocess(self, est_flow, est_cov, bl_fx: float):
-        H, W = est_flow.shape[-2:]
-        if self._score is None or (self._score.h, self._score.w) != (H, W):
-            self._score = ops.ScoreBuffers(H, W, self.device, int(getattr(self.config, "score_kernel_size", 7)))
-        return ops.dense_postproc(est_flow, est_cov, bl_fx, self.config.enforce_positive_disparity, score=self._score)
-
-    def _run(self, input_A, input_B, bl_fx: float):
-        # input_A = [t2.L, t1.L], input_B = [t2.R, t2.L]: B[1] is A[0], which the feature encoder then sees once
-        est_flow, est_cov = self.net.inference(input_A, input_B, shared=(0, 1))
-        return self._postprocess(est_flow.float(), est_cov.float(), bl_fx)
+    def _run(self, input_A, input_B, bl_fx: float) -> dict:
+        raise NotImplementedError
 
     def _outputs(self, d: dict, clone: bool):
-        c = (lambda t: t.clone() if t is not None else None) if clone else (lambda t: t)
-        depth = IStereoDepth.Output(depth=c(d["depth"]), cov=c(d["depth_cov"]), disparity=c(d["disparity"]),
-                                    disparity_uncertainty=c(d["disparity_uncertainty"]), mask=c(d["depth_mask"]))
-        match = IMatcher.Output(flow=c(d["flow"]), cov=c(d["flow_cov"]), mask=None)
-        # let the selector plugin reuse the fused scores instead of re-reading the covariance map
-        self._score.generation += 1
-        # (the token is keyed by buffer generation + map address; the covariance map must not be edited in place between
-        # estimate_pair and select_point — inference tensors carry no version counter that could detect it)
-        match._b200_score = (self._score, self._score.generation, match.cov.data_ptr())  # type: ignore[attr-defined]
-        return depth, match
-
-    @torch.inference_mode()
-    def estimate_depth(self, frame: StereoData):
-        A = frame.imageL.to(self.device, non_blocking=True)
-        B = frame.imageR.to(self.device, non_blocking=True)
-        est_flow, est_cov = self.net.inference(A, B)
-        est_flow, est_cov = est_flow.float(), est_cov.float()
-        # B = 1 call: reuse the pair kernel by duplicating the slot (slot 1 outputs are ignored)
-        d = ops.dense_postproc(torch.cat([est_flow, est_flow]), torch.cat([est_cov, est_cov]),
-                               frame.frame_baseline * frame.fx, self.config.enforce_positive_disparity, score=None)
-        return IStereoDepth.Output(depth=d["depth"], cov=d["depth_cov"], disparity=d["disparity"],
-                                   disparity_uncertainty=est_cov[0:1, :1], mask=d["depth_mask"])
+        raise NotImplementedError
 
     @torch.inference_mode()
     def estimate_pair(self, frame_t1: StereoData, frame_t2: StereoData):
@@ -212,6 +162,77 @@ class B200_FlowFormerCovFrontend(IFrontend):
             return ops.retrieve_pixels(pixel_uv.to(scalar_map.device), scalar_map)
         return scalar_map[0, ..., pixel_uv[..., 1].long(), pixel_uv[..., 0].long()]   # e.g. the CPU colour image
 
+
+class B200_FlowFormerCovFrontend(_B200_GraphedPairFrontend):
+    """FlowFormerCov stereo + flow frontend: correlation volume and window lookup on sm_90a kernels,
+    dense post-processing + keypoint scoring fused into one pass, the whole `estimate_pair` replayed as a
+    CUDA graph (like CUDAGraph_FlowFormerCovFrontend, Frontend.py:301-353).
+
+    config: weight (checkpoint path, or "synthetic[:seed]" for the deterministic stand-in), device,
+    enc_dtype / dec_dtype in {fp32, fp16, bf16}, decoder_depth, enforce_positive_disparity,
+    cuda_graph (bool), score_kernel_size (odd int; NMS window of the fused keypoint scoring, 7 in the
+    reference configs)."""
+
+    def __init__(self, config: SimpleNamespace):
+        super().__init__(config)
+        self.device = _require_cuda(config.device, "B200_FlowFormerCovFrontend")
+        sd = _load_weights(config.weight, covariance=True)
+        enc, dec = _DTYPES[config.enc_dtype], _DTYPES[config.dec_dtype]
+        # MACVO_Fast (enc fp16 / dec bf16, Config/Experiment/MACVO/MACVO_Fast.yaml:8-9) exists because half-precision tensor
+        # cores are the fast path on the GPUs MAC-VO targets. The TF32 pipeline of this class (own kernels + TF32
+        # cuDNN / cuBLAS) is ~4x closer to exact arithmetic than the
+        # reference's own fp16 / bf16 run (flow 9e-4 vs 3.3e-3 of its scale, tests/test_gpu_pipeline.py::test_fast_config_*),
+        # so half-precision configs are served by it unless `half_precision: native` asks for the literal dtypes.
+        self.half_precision = getattr(config, "half_precision", "tf32")
+        if self.half_precision == "tf32":
+            enc = dec = torch.float32
+        self.net = FlowFormerCovNet(sd, self.device, enc, dec, decoder_depth=config.decoder_depth)
+        # the reference frontend enables TF32 tensor cores for the dense layers (Frontend.py:275-277)
+        torch.backends.cuda.matmul.allow_tf32 = True
+        torch.backends.cudnn.allow_tf32 = True
+        torch.set_float32_matmul_precision("medium")
+        self._score: ops.ScoreBuffers | None = None
+
+    @property
+    def provide_cov(self) -> tuple[bool, bool]:
+        return True, True
+
+    # ---- (a7) + fused (a8) scoring ---------------------------------------------------------------
+    def _postprocess(self, est_flow, est_cov, bl_fx: float):
+        H, W = est_flow.shape[-2:]
+        if self._score is None or (self._score.h, self._score.w) != (H, W):
+            self._score = ops.ScoreBuffers(H, W, self.device, int(getattr(self.config, "score_kernel_size", 7)))
+        return ops.dense_postproc(est_flow, est_cov, bl_fx, self.config.enforce_positive_disparity, score=self._score)
+
+    def _run(self, input_A, input_B, bl_fx: float):
+        # input_A = [t2.L, t1.L], input_B = [t2.R, t2.L]: B[1] is A[0], which the feature encoder then sees once
+        est_flow, est_cov = self.net.inference(input_A, input_B, shared=(0, 1))
+        return self._postprocess(est_flow.float(), est_cov.float(), bl_fx)
+
+    def _outputs(self, d: dict, clone: bool):
+        c = (lambda t: t.clone() if t is not None else None) if clone else (lambda t: t)
+        depth = IStereoDepth.Output(depth=c(d["depth"]), cov=c(d["depth_cov"]), disparity=c(d["disparity"]),
+                                    disparity_uncertainty=c(d["disparity_uncertainty"]), mask=c(d["depth_mask"]))
+        match = IMatcher.Output(flow=c(d["flow"]), cov=c(d["flow_cov"]), mask=None)
+        # let the selector plugin reuse the fused scores instead of re-reading the covariance map
+        self._score.generation += 1
+        # (the token is keyed by buffer generation + map address; the covariance map must not be edited in place between
+        # estimate_pair and select_point — inference tensors carry no version counter that could detect it)
+        match._b200_score = (self._score, self._score.generation, match.cov.data_ptr())  # type: ignore[attr-defined]
+        return depth, match
+
+    @torch.inference_mode()
+    def estimate_depth(self, frame: StereoData):
+        A = frame.imageL.to(self.device, non_blocking=True)
+        B = frame.imageR.to(self.device, non_blocking=True)
+        est_flow, est_cov = self.net.inference(A, B)
+        est_flow, est_cov = est_flow.float(), est_cov.float()
+        # B = 1 call: reuse the pair kernel by duplicating the slot (slot 1 outputs are ignored)
+        d = ops.dense_postproc(torch.cat([est_flow, est_flow]), torch.cat([est_cov, est_cov]),
+                               frame.frame_baseline * frame.fx, self.config.enforce_positive_disparity, score=None)
+        return IStereoDepth.Output(depth=d["depth"], cov=d["depth_cov"], disparity=d["disparity"],
+                                   disparity_uncertainty=est_cov[0:1, :1], mask=d["depth_mask"])
+
     @classmethod
     def is_valid_config(cls, config: SimpleNamespace | None) -> None:
         spec = {
@@ -229,6 +250,60 @@ class B200_FlowFormerCovFrontend(IFrontend):
                     "score_kernel_size": lambda k: isinstance(k, int) and k % 2 == 1 and 1 <= k <= 15}
         if config is not None:
             spec.update({k: v for k, v in optional.items() if hasattr(config, k)})
+        cls._enforce_config_spec(config, spec)
+
+
+class B200_FlowFormerFrontend(_B200_GraphedPairFrontend):
+    """The covariance-free frontend of the Vanilla ablation (Config/Experiment/MACVO/Ablation_Study/TartanAirv2_Vanilla.yaml):
+    FrontendCompose of FlowFormerDepth + FlowFormerMatcher, which load the same plain FlowFormer checkpoint (fp32, decoder
+    depth 12, configs/submission.py:32). One network serves both: `estimate_pair` is one B = 2 pass, graphed like
+    B200_FlowFormerCovFrontend's, `estimate_depth` one eager B = 1 pass.
+
+    Outputs as the reference's: depth / disparity (1,1,H,W) with disparity = |flow_x| and depth = (bl * fx) / disparity
+    (StereoDepth.py:122-128), flow (1,2,H,W); every covariance, the disparity uncertainty and the masks are None.
+    The TF32 flags are left as the process has them (the reference classes do not touch them), so the network runs its
+    strict fp32 loop under torch's defaults and its TF32 loop when the caller allows TF32.
+
+    config: weight (plain FlowFormer or FlowFormerCov checkpoint path, or "synthetic[:seed]"), device, cuda_graph (optional
+    bool, default True)."""
+
+    DECODER_DEPTH = 12
+
+    def __init__(self, config: SimpleNamespace):
+        super().__init__(config)
+        self.device = _require_cuda(config.device, "B200_FlowFormerFrontend")
+        self.net = FlowFormerCovNet(_load_weights(config.weight, covariance=False), self.device,
+                                    decoder_depth=self.DECODER_DEPTH, covariance=False)
+
+    @property
+    def provide_cov(self) -> tuple[bool, bool]:
+        return False, False
+
+    def _run(self, input_A, input_B, bl_fx: float):
+        est_flow, _ = self.net.inference(input_A, input_B, shared=(0, 1))
+        return ops.dense_postproc(est_flow, None, bl_fx)
+
+    def _outputs(self, d: dict, clone: bool):
+        c = (lambda t: t.clone()) if clone else (lambda t: t)
+        return (IStereoDepth.Output(depth=c(d["depth"]), disparity=c(d["disparity"])),
+                IMatcher.Output(flow=c(d["flow"])))
+
+    @torch.inference_mode()
+    def estimate_depth(self, frame: StereoData):
+        A = frame.imageL.to(self.device, non_blocking=True)
+        B = frame.imageR.to(self.device, non_blocking=True)
+        est_flow, _ = self.net.inference(A, B)
+        d = ops.dense_postproc(est_flow, None, frame.frame_baseline * frame.fx)
+        return IStereoDepth.Output(depth=d["depth"], disparity=d["disparity"])
+
+    @classmethod
+    def is_valid_config(cls, config: SimpleNamespace | None) -> None:
+        spec = {
+            "weight": lambda s: isinstance(s, str),
+            "device": lambda s: isinstance(s, str) and "cuda" in s,
+        }
+        if config is not None and hasattr(config, "cuda_graph"):
+            spec["cuda_graph"] = lambda b: isinstance(b, bool)
         cls._enforce_config_spec(config, spec)
 
 
@@ -680,15 +755,26 @@ class B200_FilterCompose(IObservationFilter):
             IObservationFilter.is_valid_config(filter_arg)
 
 
-def observe_ext(outlier_filter) -> dict | None:
-    """`macvo_observe_pack`'s extension for an outlier filter (None: CovarianceSanityFilter alone, which observe_kernel
-    always applies). Raises for a filter the device path cannot run, or a chain without the sanity filter."""
-    if outlier_filter is None:
-        return None
+def check_sanity_chain(outlier_filter, covariance_finite: bool = False) -> None:
+    """The device observation path always applies CovarianceSanityFilter, so the outlier filter must contain
+    B200_CovarianceSanityFilter; raises otherwise. covariance_finite: the covariance model only produces finite
+    covariances (B200_NoCovariance: identities, finite under any modifier), so the always-on filter cannot drop a row and
+    a chain without it (the Vanilla ablation's [SimpleDepthFilter]) means the same thing on the device."""
+    if outlier_filter is None or covariance_finite:
+        return
     chain = outlier_filter.filters if isinstance(outlier_filter, B200_FilterCompose) else [outlier_filter]
     if not any(isinstance(f, B200_CovarianceSanityFilter) for f in chain):
         raise ValueError("the device observation path always applies CovarianceSanityFilter: the outlier filter must "
                          "contain B200_CovarianceSanityFilter")
+
+
+def observe_ext(outlier_filter, covariance_finite: bool = False) -> dict | None:
+    """`macvo_observe_pack`'s extension for an outlier filter (None: CovarianceSanityFilter alone, which observe_kernel
+    always applies). Raises for a filter the device path cannot run, or a chain without the sanity filter (unless
+    `covariance_finite`, see `check_sanity_chain`)."""
+    if outlier_filter is None:
+        return None
+    check_sanity_chain(outlier_filter, covariance_finite)
     if not hasattr(outlier_filter, "observe_ext"):
         raise ValueError(f"{type(outlier_filter).__name__} has no device implementation")
     return outlier_filter.observe_ext()
@@ -934,6 +1020,7 @@ class B200_TartanMotionNet(IMotionModel):
 
 PLUGINS = {
     "frontend": B200_FlowFormerCovFrontend,
+    "frontend_plain": B200_FlowFormerFrontend,
     "keypoint": B200_CovAwareSelector_NoDepth,
     "keypoint_depth": B200_CovAwareSelector,
     "mappoint": B200_MappingPointSelector,
