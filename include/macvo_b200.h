@@ -529,6 +529,23 @@ size_t macvo_posenet_head_floats(void);
 int macvo_posenet_head(const float* fc1_out, const float* head_blob, const double* prev_pose, float* motion,
                        double* next_pose, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * (f6) TartanVOMatcher's PWC-Net (PWCDCNet_Adapted, Module/Network/PWCNet/pwc/pwc_model_tartanvo.py:64-297): warp +
+ *      correlation + LeakyReLU(0.1) of one pyramid level — replaces warp() (:176-212), FunctionCorrelation and the
+ *      leakyRELU after it (:230-232, 259-260), i.e. the cupy kernels of correlation.py:35-102, 277-318.
+ * f1, f2 (batch, channels, H, W) fp32; flow (batch, 2, H, W) fp32, or NULL = no warp (level 6).
+ * g = f2 when flow is NULL, else g[c,y,x] = grid_sample(f2, (x + s*flow_x, y + s*flow_y))[c] * m(y,x) (s = flow_scale,
+ *      bilinear, zeros padding, align_corners=True; m = the same sampling of ones, 0 where < 0.9999, 1 where > 0). Tap
+ *      positions, weights and m are computed in fp32 in the reference's order; a non-finite position or one beyond
+ *      +-2^24 has no in-bounds tap (sample 0, m 0).
+ * out (batch, out_channels, H, W) fp32: channels [out_offset, out_offset + 81) only are written,
+ *      out[out_offset + (dy+4)*9 + (dx+4), y, x] = LeakyReLU_0.1((1/C) sum_c f1[c,y,x] g[c,y+dy,x+dx]), g = 0 outside the image.
+ * MACVO_E_ARG (nothing launched): a NULL f1 / f2 / out, a size <= 0, out_offset < 0 or out_offset + 81 > out_channels.
+ */
+int macvo_pwc_warp_corr(const float* f1, const float* f2, const float* flow, float flow_scale,
+                        int batch, int channels, int height, int width,
+                        float* out, int out_channels, int out_offset, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

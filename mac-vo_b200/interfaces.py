@@ -10,7 +10,7 @@ provide the same names, signatures and error behaviour for the methods the hot p
 
     IFrontend            Module/Frontend/Frontend.py:38-118
     IStereoDepth.Output  Module/Frontend/StereoDepth.py:35-40
-    IMatcher.Output      Module/Frontend/Matching.py:23-40
+    IMatcher             Module/Frontend/Matching.py:20-70 (Output, provide_cov, forward, estimate)
     IKeypointSelector    Module/KeypointSelector.py:17-48
     ICovariance2to3      Module/Covariance/Project2to3.py:16-44
     IMotionModel         Module/MotionModel.py:15-41
@@ -132,6 +132,7 @@ class IStereoDepth(ABC, _Registry):
 
 
 class IMatcher(ABC, _Registry):
+    """Module/Frontend/Matching.py:20-70"""
     _IS_INTERFACE = True
 
     @dataclass
@@ -139,6 +140,20 @@ class IMatcher(ABC, _Registry):
         flow: torch.Tensor
         cov: torch.Tensor | None = None
         mask: torch.Tensor | None = None
+
+    def __init__(self, config: SimpleNamespace):
+        self.config = config
+
+    @property
+    @abstractmethod
+    def provide_cov(self) -> bool: ...
+
+    @abstractmethod
+    def forward(self, frame_t1: StereoData, frame_t2: StereoData) -> "IMatcher.Output": ...
+
+    def estimate(self, frame_t1: StereoData, frame_t2: StereoData) -> "IMatcher.Output":
+        with torch.no_grad(), torch.inference_mode():
+            return self.forward(frame_t1, frame_t2)
 
 
 class IFrontend(ABC, _Registry):

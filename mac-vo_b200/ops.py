@@ -123,6 +123,8 @@ EXPORTS = {
                            + [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "macvo_posenet_head_floats": (C.c_size_t, []),
     "macvo_posenet_head": (C.c_int, [C.c_void_p] * 6),
+    "macvo_pwc_warp_corr": (C.c_int, [C.c_void_p] * 3 + [C.c_float] + [C.c_int] * 4 + [C.c_void_p] + [C.c_int] * 2
+                            + [C.c_void_p]),
 }
 
 
@@ -1453,3 +1455,37 @@ def posenet_head(fc1_out: Tensor, head_blob: Tensor, prev_pose: Tensor, motion: 
     _check(load_library().macvo_posenet_head(h.data_ptr(), blob.data_ptr(), pp.data_ptr(), motion.data_ptr(),
                                              next_pose.data_ptr(), _stream()), "macvo_posenet_head")
     LAUNCHES[0] += 1
+
+
+# ------------------------------------------------------------------------------------------------
+# (f6) TartanVOMatcher's PWC-Net: warp + correlation + LeakyReLU of one level (csrc/pwc_corr.cu)
+# ------------------------------------------------------------------------------------------------
+PWC_DISPLACEMENTS = 81
+
+
+def pwc_warp_corr(f1: Tensor, f2: Tensor, flow: Tensor | None, scale: float, out: Tensor, out_offset: int) -> Tensor:
+    """LeakyReLU_0.1(correlation(f1, warp(f2, scale * flow))) of PWCDCNet_Adapted (no warp when flow is None) written into
+    channels [out_offset, out_offset + 81) of out (B, C_out, H, W); f1, f2 (B, C, H, W), flow (B, 2, H, W). Returns out."""
+    a = _dev(f1, torch.float32, "pwc_warp_corr f1")
+    b = _dev(f2, torch.float32, "pwc_warp_corr f2")
+    if a.dim() != 4 or b.shape != a.shape:
+        raise MacvoB200Error(f"pwc_warp_corr: f1 {tuple(a.shape)} and f2 {tuple(b.shape)} must be the same (B,C,H,W)")
+    B, Cc, H, W = a.shape
+    fl = None
+    if flow is not None:
+        fl = _dev(flow, torch.float32, "pwc_warp_corr flow")
+        if tuple(fl.shape) != (B, 2, H, W):
+            raise MacvoB200Error(f"pwc_warp_corr: flow {tuple(fl.shape)} must be ({B},2,{H},{W})")
+    if not (isinstance(out, Tensor) and out.is_cuda and out.dtype == torch.float32 and out.is_contiguous()
+            and out.dim() == 4 and out.shape[0] == B and tuple(out.shape[2:]) == (H, W)):
+        raise MacvoB200Error(f"pwc_warp_corr: out must be a contiguous ({B},C_out,{H},{W}) fp32 CUDA tensor")
+    if not 0 <= out_offset <= out.shape[1] - PWC_DISPLACEMENTS:
+        raise MacvoB200Error(f"pwc_warp_corr: channels [{out_offset}, {out_offset + PWC_DISPLACEMENTS}) exceed out's {out.shape[1]}")
+    if b.device != a.device or out.device != a.device or (fl is not None and fl.device != a.device):
+        raise MacvoB200Error("pwc_warp_corr: all tensors must be on one device")
+    rc = load_library().macvo_pwc_warp_corr(a.data_ptr(), b.data_ptr(), fl.data_ptr() if fl is not None else None,
+                                            float(scale), B, Cc, H, W, out.data_ptr(), out.shape[1], int(out_offset),
+                                            _stream())
+    _check(rc, "macvo_pwc_warp_corr")
+    LAUNCHES[0] += 1
+    return out

@@ -18,6 +18,7 @@
     B200_MotionInterpolate           IMapProcessor      replaces MotionInterpolate (MapProcessor.py:52-79)
     B200_TwoFrame_PGO                IOptimizer         replaces TwoFrame_PGO (Optimization/TwoFramePGO/Optimizer.py:23-108)
     B200_TartanMotionNet             IMotionModel       replaces TartanMotionNet (MotionModel.py:89-116)
+    B200_TartanVOMatcher             IMatcher           replaces TartanVOMatcher (Frontend/Matching.py:199-230)
 
 Same constructor signature (`__init__(config: SimpleNamespace)`), same `is_valid_config` contract
 (unknown keys are an error), same argument meaning and return types as the classes they replace; class
@@ -37,6 +38,7 @@ import torch
 from . import interfaces as _local
 from . import ops
 from . import posenet
+from . import pwcnet
 from .flowformer_cov import FlowFormerCovNet, synthetic_state_dict
 
 _REF = _local.reference_available()
@@ -1018,6 +1020,124 @@ class B200_TartanMotionNet(IMotionModel):
         })
 
 
+# ================================================================================================
+# Matcher
+# ================================================================================================
+class B200_TartanVOMatcher(IMatcher):
+    """Replacement of TartanVOMatcher (Module/Frontend/Matching.py:199-230), the optical flow of the TartanVO baseline
+    (Config/Experiment/Baseline/TartanVO/TartanVOStereo.yaml): TartanVO's PWC-Net (pwcnet.PWCFlowNet) with its warp +
+    correlation in macvo_pwc_warp_corr and its convolutions on cuDNN; no cupy, cv2 or host round trip.
+
+    config: weight (checkpoint path — only its `module.flowNet.*` tensors are used — or "synthetic[:seed]"), device (CUDA),
+    optional cuda_graph (default true: crop, network and output shaping are captured as one CUDA graph on the first call
+    and replayed after; the image shape must then stay the same).
+
+    `forward` returns what the reference returns (TartanStereoVOMatch.inference, StereoVO_Interface.py:124-151, and
+    Matching.py:213-223), as fresh tensors on config.device:
+      * flow (1,2,H,W) fp32: both left images centre-cropped to (H//64*64, W//64*64), raw (not normalised), the network's
+        flow2 / 0.05, nearest-upsampled x4 and NaN-padded to the frame size;
+      * mask (1,1,h64,w64) bool, built like the reference's from the *cropped* flow before padding: True on
+        [ph:-ph, pw:-pw] with ph, pw the crop margins — all False when H or W is a multiple of 64 (INTEGRATION.md);
+      * a batch other than 1, or an odd total margin, raises AssertionError like the reference."""
+
+    def __init__(self, config: SimpleNamespace):
+        super().__init__(config)
+        self.device = _require_cuda(config.device, "B200_TartanVOMatcher")
+        w = config.weight
+        if isinstance(w, str) and w.startswith("synthetic"):
+            sd = pwcnet.synthetic_pwc_state_dict(int(w.split(":")[1]) if ":" in w else 0)
+        else:
+            sd = pwcnet.load_checkpoint(w)
+        self.net = pwcnet.PWCFlowNet(sd, self.device)
+        self.use_graph = bool(getattr(config, "cuda_graph", True))
+        self._replay = None
+        self._static: dict = {}
+
+    @property
+    def provide_cov(self) -> bool:
+        return False
+
+    @staticmethod
+    def geometry(H: int, W: int) -> tuple[tuple[int, int], tuple[int, int]]:
+        """((crop margin y, x), (h64, w64)) of getCropMargin (StereoVO_Interface.py:107-115), checked like padTo"""
+        h64, w64 = H // 64 * 64, W // 64 * 64
+        if h64 == 0 or w64 == 0:
+            raise ValueError(f"B200_TartanVOMatcher: a {H}x{W} image is smaller than PWC-Net's 64x64 input granule")
+        for size, crop, dim in ((H, h64, -2), (W, w64, -1)):
+            assert (size - crop) % 2 == 0, \
+                f"Can only handle even padding. Target_size={size}, Actual_size={crop} on dim {dim}."
+        return ((H - h64) // 2, (W - w64) // 2), (h64, w64)
+
+    def _run(self, images: torch.Tensor, flow_out: torch.Tensor, margin, crop) -> None:
+        """images (2,3,H,W) -> flow_out (1,2,H,W): crop, network, / 0.05, nearest x4 into the NaN-padded frame"""
+        (my, mx), (h64, w64) = margin, crop
+        flow2 = self.net.flow2(images[:, :, my:my + h64, mx:mx + w64].contiguous())
+        up = (flow2 / pwcnet.FLOW_NORM).repeat_interleave(4, dim=-2).repeat_interleave(4, dim=-1)
+        flow_out[:, :, my:my + h64, mx:mx + w64].copy_(up)
+
+    def _capture(self, run):
+        """capture `run` as a CUDA graph (after a warm-up run outside the capture, for cuDNN's algorithm choice); returns a
+        callable that replays it"""
+        side = torch.cuda.Stream(self.device)
+        side.wait_stream(torch.cuda.current_stream())
+        with torch.cuda.stream(side):
+            run()
+        torch.cuda.current_stream().wait_stream(side)
+        graph = torch.cuda.CUDAGraph()
+        n0 = ops.LAUNCHES[0]
+        with torch.cuda.graph(graph):
+            run()
+        launches = ops.LAUNCHES[0] - n0
+
+        def replay():
+            graph.replay()
+            ops.LAUNCHES[0] += launches
+        return replay
+
+    def forward(self, frame_t1: StereoData, frame_t2: StereoData) -> IMatcher.Output:
+        img1, img2 = frame_t1.imageL, frame_t2.imageL
+        assert img1.size(0) == 1 and img2.size(0) == 1, "The interface will not handle batch dimension correctly."
+        H, W = img1.shape[-2:]
+        assert tuple(img2.shape[-2:]) == (H, W), "both frames must have the same image size"
+        st = self._static
+        if self._replay is not None:
+            assert (H, W) == st["shape"], f"image shape changed since the CUDA graph was captured: {(H, W)} != {st['shape']}"
+        else:
+            margin, crop = self.geometry(H, W)
+            mask = torch.zeros((1, 1) + crop, dtype=torch.bool, device=self.device)
+            ph, pw = margin                              # (frame size - flow size) // 2 of Matching.py:217-218
+            mask[..., ph:-ph, pw:-pw] = True             # the reference's slice: empty when a margin is 0
+            st = self._static = {"shape": (H, W), "margin": margin, "crop": crop, "mask": mask,
+                                 "images": torch.empty((2, 3, H, W), dtype=torch.float32, device=self.device),
+                                 "flow": torch.full((1, 2, H, W), float("nan"), dtype=torch.float32, device=self.device)}
+        st["images"][0:1].copy_(img1, non_blocking=True)
+        st["images"][1:2].copy_(img2, non_blocking=True)
+        run = lambda: self._run(st["images"], st["flow"], st["margin"], st["crop"])
+        # deterministic cuDNN algorithms (the transposed convolutions would otherwise be free to accumulate with atomics), so
+        # that a graph replay, the first call and cuda_graph: false give the same bits; TF32 and the other flags as they are
+        with torch.backends.cudnn.flags(enabled=torch.backends.cudnn.enabled, benchmark=torch.backends.cudnn.benchmark,
+                                        benchmark_limit=torch.backends.cudnn.benchmark_limit, deterministic=True,
+                                        allow_tf32=torch.backends.cudnn.allow_tf32):
+            if not self.use_graph:
+                run()
+            elif self._replay is None:
+                self._replay = self._capture(run)
+                self._replay()
+            else:
+                self._replay()
+        return IMatcher.Output(flow=st["flow"].clone(), mask=st["mask"].clone())
+
+    @classmethod
+    def is_valid_config(cls, config: SimpleNamespace | None) -> None:
+        spec = {
+            "weight": lambda f: isinstance(f, str),
+            "device": lambda dev: isinstance(dev, str) and "cuda" in dev,
+        }
+        if config is not None and "cuda_graph" in vars(config):
+            spec["cuda_graph"] = lambda b: isinstance(b, bool)
+        cls._enforce_config_spec(config, spec)
+
+
 PLUGINS = {
     "frontend": B200_FlowFormerCovFrontend,
     "frontend_plain": B200_FlowFormerFrontend,
@@ -1033,4 +1153,5 @@ PLUGINS = {
     "postprocess": B200_MotionInterpolate,
     "optimizer": B200_TwoFrame_PGO,
     "motion": B200_TartanMotionNet,
+    "matcher_tartanvo": B200_TartanVOMatcher,
 }
