@@ -546,6 +546,23 @@ int macvo_pwc_warp_corr(const float* f1, const float* f2, const float* flow, flo
                         int batch, int channels, int height, int width,
                         float* out, int out_channels, int out_offset, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * (f7) TartanVODepth's full-resolution heads and depth conversion (StereoCovNet(exp=False, decoder="hourglass"),
+ *      Module/Network/StereoCov/{StereoNet,decoder,network}.py): for the disparity head (xd) and, when xc is not NULL, the
+ *      covariance head (xc), with K = [x | cat0] (64 + 64 channels):
+ *      out = conv_c13(relu(conv_c12(relu(deconv_c11(K))))) (+ relu on the covariance head), then disp = out_d / 0.02,
+ *      depth = (1 / disp) * bf, var = bf2 * ((out_c / disp^2) / disp^2), all fp32 with IEEE division.
+ * xd, xc, cat0 (1, 64, h2, w2) fp32 contiguous; w11_* (4 chunks, 4 phases, 4 taps, 64, 32) fp32, tf32-rounded
+ *      (stereonet.arrange_head); small_* b11 (64) | w12 (16 x 64) | b12 (16) | w13 (16) | b13 (1) fp32.
+ * depth, var (height, width) fp32: only [margin_y, margin_y + 2 h2) x [margin_x, margin_x + 2 w2) is written; var is
+ *      not touched when xc is NULL. Runs the deconvolution on TF32 tensor cores (the caller decides that TF32 is allowed).
+ * MACVO_E_ARG (nothing launched): a NULL xd / cat0 / w11_d / small_d / depth, xc without w11_c / small_c / var, a size
+ *      <= 0, a negative margin, a crop beyond the frame, or a weight blob not 16-byte aligned.
+ */
+int macvo_stereo_head(const float* xd, const float* xc, const float* cat0, int h2, int w2, const float* w11_d,
+                      const float* small_d, const float* w11_c, const float* small_c, float bf, float bf2, int margin_y,
+                      int margin_x, int height, int width, float* depth, float* var, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -9,7 +9,7 @@ When MAC-VO is not importable (no MAC-VO tree on the path) the minimal mirrors b
 provide the same names, signatures and error behaviour for the methods the hot path uses:
 
     IFrontend            Module/Frontend/Frontend.py:38-118
-    IStereoDepth.Output  Module/Frontend/StereoDepth.py:35-40
+    IStereoDepth         Module/Frontend/StereoDepth.py:18-50 (Output, provide_cov, estimate)
     IMatcher             Module/Frontend/Matching.py:20-70 (Output, provide_cov, forward, estimate)
     IKeypointSelector    Module/KeypointSelector.py:17-48
     ICovariance2to3      Module/Covariance/Project2to3.py:16-44
@@ -120,6 +120,7 @@ class StereoData:
 
 
 class IStereoDepth(ABC, _Registry):
+    """Module/Frontend/StereoDepth.py:18-50"""
     _IS_INTERFACE = True
 
     @dataclass
@@ -129,6 +130,16 @@ class IStereoDepth(ABC, _Registry):
         cov: torch.Tensor | None = None
         mask: torch.Tensor | None = None
         disparity_uncertainty: torch.Tensor | None = None
+
+    def __init__(self, config: SimpleNamespace):
+        self.config = config
+
+    @property
+    @abstractmethod
+    def provide_cov(self) -> bool: ...
+
+    @abstractmethod
+    def estimate(self, frame: StereoData) -> "IStereoDepth.Output": ...
 
 
 class IMatcher(ABC, _Registry):

@@ -125,6 +125,8 @@ EXPORTS = {
     "macvo_posenet_head": (C.c_int, [C.c_void_p] * 6),
     "macvo_pwc_warp_corr": (C.c_int, [C.c_void_p] * 3 + [C.c_float] + [C.c_int] * 4 + [C.c_void_p] + [C.c_int] * 2
                             + [C.c_void_p]),
+    "macvo_stereo_head": (C.c_int, [C.c_void_p] * 3 + [C.c_int] * 2 + [C.c_void_p] * 4 + [C.c_float] * 2 + [C.c_int] * 4
+                          + [C.c_void_p] * 3),
 }
 
 
@@ -1489,3 +1491,61 @@ def pwc_warp_corr(f1: Tensor, f2: Tensor, flow: Tensor | None, scale: float, out
     _check(rc, "macvo_pwc_warp_corr")
     LAUNCHES[0] += 1
     return out
+
+
+# ------------------------------------------------------------------------------------------------
+# (f7) TartanVODepth: both full-resolution heads + the depth conversion (csrc/stereo_head.cu)
+# ------------------------------------------------------------------------------------------------
+STEREO_HEAD_SMALL = 64 + 16 * 64 + 16 + 16 + 1          # b11 | w12 (16 x 64) | b12 | w13 | b13
+
+
+def stereo_head(xd: Tensor, xc: Tensor | None, cat0: Tensor, w11_d: Tensor, small_d: Tensor, w11_c: Tensor | None,
+                small_c: Tensor | None, bf: float, margin: tuple[int, int], depth: Tensor, var: Tensor | None) -> None:
+    """TartanVODepth's heads from the conv_c10 outputs xd (disparity decoder) and xc (covariance decoder, or None) and cat0,
+    all (1, 64, h2, w2), into the crop region [my, my + 2 h2) x [mx, mx + 2 w2) of depth / var (1, 1, H, W): deconv_c11 on
+    TF32 tensor cores (w11_* from stereonet.arrange_head), conv_c12, conv_c13, / 0.02 and StereoCovNet.inference. The
+    deconvolution is a TF32 one, so the call is refused unless torch.backends.cudnn.allow_tf32 is set (the flag under which
+    cuDNN would run it in TF32 too)."""
+    if not torch.backends.cudnn.allow_tf32:
+        raise MacvoB200Error("stereo_head: runs deconv_c11 in TF32, but torch.backends.cudnn.allow_tf32 is False")
+    if (xc is None) != (var is None) or (xc is None) != (w11_c is None) or (xc is None) != (small_c is None):
+        raise MacvoB200Error("stereo_head: xc, w11_c, small_c and var go together (all or none)")
+    a = _dev(xd, torch.float32, "stereo_head xd")
+    k = _dev(cat0, torch.float32, "stereo_head cat0")
+    if a.dim() != 4 or a.shape[:2] != (1, 64) or k.shape != a.shape:
+        raise MacvoB200Error(f"stereo_head: xd {tuple(a.shape)} and cat0 {tuple(k.shape)} must both be (1,64,h2,w2)")
+    h2, w2 = a.shape[-2:]
+    heads = [(a, w11_d, small_d)]
+    if xc is not None:
+        c = _dev(xc, torch.float32, "stereo_head xc")
+        if c.shape != a.shape:
+            raise MacvoB200Error(f"stereo_head: xc {tuple(c.shape)} must be {tuple(a.shape)}")
+        heads.append((c, w11_c, small_c))
+    for _, w, sm in heads:
+        if not (isinstance(w, Tensor) and w.is_cuda and w.dtype == torch.float32 and w.is_contiguous()
+                and tuple(w.shape) == (4, 4, 4, 64, 32)):
+            raise MacvoB200Error("stereo_head: w11 must be a contiguous (4,4,4,64,32) fp32 CUDA tensor (arrange_head)")
+        if not (isinstance(sm, Tensor) and sm.is_cuda and sm.dtype == torch.float32 and sm.is_contiguous()
+                and sm.numel() == STEREO_HEAD_SMALL):
+            raise MacvoB200Error(f"stereo_head: small must be a contiguous fp32 CUDA tensor of {STEREO_HEAD_SMALL} floats")
+    outs = [depth] + ([var] if var is not None else [])
+    for o in outs:
+        if not (isinstance(o, Tensor) and o.is_cuda and o.dtype == torch.float32 and o.is_contiguous() and o.dim() == 4
+                and o.shape[:2] == (1, 1)):
+            raise MacvoB200Error("stereo_head: depth / var must be contiguous (1,1,H,W) fp32 CUDA tensors")
+    H, W = depth.shape[-2:]
+    if var is not None and var.shape != depth.shape:
+        raise MacvoB200Error(f"stereo_head: var {tuple(var.shape)} must be {tuple(depth.shape)}")
+    my, mx = int(margin[0]), int(margin[1])
+    if my < 0 or mx < 0 or my + 2 * h2 > H or mx + 2 * w2 > W:
+        raise MacvoB200Error(f"stereo_head: a {2 * h2}x{2 * w2} crop at ({my}, {mx}) does not fit a {H}x{W} frame")
+    devs = {t.device for t in [a, k, *outs] + [x for _, w, s in heads for x in (w, s)] + ([heads[1][0]] if xc is not None else [])}
+    if len(devs) != 1:
+        raise MacvoB200Error("stereo_head: all tensors must be on one device")
+    bf = float(bf)
+    ptr = lambda t: t.data_ptr() if t is not None else None
+    rc = load_library().macvo_stereo_head(a.data_ptr(), ptr(heads[1][0]) if xc is not None else None, k.data_ptr(), h2, w2,
+                                          w11_d.data_ptr(), small_d.data_ptr(), ptr(w11_c), ptr(small_c), bf, bf * bf,
+                                          my, mx, H, W, depth.data_ptr(), ptr(var), _stream())
+    _check(rc, "macvo_stereo_head")
+    LAUNCHES[0] += 1

@@ -19,6 +19,7 @@
     B200_TwoFrame_PGO                IOptimizer         replaces TwoFrame_PGO (Optimization/TwoFramePGO/Optimizer.py:23-108)
     B200_TartanMotionNet             IMotionModel       replaces TartanMotionNet (MotionModel.py:89-116)
     B200_TartanVOMatcher             IMatcher           replaces TartanVOMatcher (Frontend/Matching.py:199-230)
+    B200_TartanVODepth               IStereoDepth       replaces TartanVODepth (Frontend/StereoDepth.py:186-229)
 
 Same constructor signature (`__init__(config: SimpleNamespace)`), same `is_valid_config` contract
 (unknown keys are an error), same argument meaning and return types as the classes they replace; class
@@ -39,6 +40,7 @@ from . import interfaces as _local
 from . import ops
 from . import posenet
 from . import pwcnet
+from . import stereonet
 from .flowformer_cov import FlowFormerCovNet, synthetic_state_dict
 
 _REF = _local.reference_available()
@@ -1138,6 +1140,153 @@ class B200_TartanVOMatcher(IMatcher):
         cls._enforce_config_spec(config, spec)
 
 
+
+# ================================================================================================
+# Stereo depth
+# ================================================================================================
+class B200_TartanVODepth(IStereoDepth):
+    """Replacement of TartanVODepth (Module/Frontend/StereoDepth.py:186-229), the stereo depth and covariance of the TartanVO
+    baseline (Config/Experiment/Baseline/TartanVO/TartanVOStereo.yaml): StereoCovNet(exp=False, decoder="hourglass")
+    (stereonet.StereoCovNetDevice) with its convolutions on cuDNN and both full-resolution heads plus the depth conversion
+    in macvo_stereo_head.
+
+    config: weight (a TartanVO_depth_cov.pth-style checkpoint, `module.` prefix optional, or "synthetic[:seed]"), device
+    (CUDA), cov_mode ("Est" or "None"), optional cuda_graph (default true: crop, normalisation, network and heads are
+    captured as one CUDA graph per image shape on the first call and replayed after; the image shape and baseline * fx
+    must then stay the same).
+
+    `estimate` returns what the reference returns, as fresh tensors on config.device: depth (1,1,H,W) and, under "Est", cov
+    (the depth variance, (1,1,H,W)), computed on the centre crop (H//64*64, W//64*64) and NaN outside it. Under "None" the
+    covariance decoder is not run at all (the reference computes it and discards it; the depth is the same).
+    The heads run in macvo_stereo_head when torch.backends.cudnn.allow_tf32 is set (torch's default, under which cuDNN runs
+    the reference's deconvolution in TF32 too), else as torch ops; the flag is read, never changed."""
+
+    MEAN = stereonet.IMG_MEAN
+    STD = stereonet.IMG_STD
+
+    def __init__(self, config: SimpleNamespace):
+        super().__init__(config)
+        self.device = _require_cuda(config.device, "B200_TartanVODepth")
+        w = config.weight
+        if isinstance(w, str) and w.startswith("synthetic"):
+            sd = stereonet.synthetic_stereo_state_dict(int(w.split(":")[1]) if ":" in w else 0)
+        else:
+            sd = stereonet.load_checkpoint(w)
+        self.net = stereonet.StereoCovNetDevice(sd, self.device)
+        self.est_cov = config.cov_mode == "Est"
+        self.use_graph = bool(getattr(config, "cuda_graph", True))
+        self._mean = torch.tensor(self.MEAN, dtype=torch.float32, device=self.device).view(1, 3, 1, 1)
+        self._std = torch.tensor(self.STD, dtype=torch.float32, device=self.device).view(1, 3, 1, 1)
+        self._replay = None
+        self._static: dict = {}
+
+    @property
+    def provide_cov(self) -> bool:
+        return self.config.cov_mode == "Est"
+
+    @staticmethod
+    def geometry(H: int, W: int) -> tuple[tuple[int, int], tuple[int, int]]:
+        """((crop margin y, x), (h64, w64)) of StereoFeature.getCropMargin (network.py:22-31), checked like padTo"""
+        h64, w64 = H // 64 * 64, W // 64 * 64
+        if h64 < stereonet.MIN_CROP or w64 < stereonet.MIN_CROP:
+            raise ValueError(f"B200_TartanVODepth: a {H}x{W} image gives a {h64}x{w64} crop; StereoNet7's 64x64 average "
+                             f"pooling at 1/4 resolution needs a crop of at least {stereonet.MIN_CROP}x{stereonet.MIN_CROP}")
+        for size, crop, dim in ((H, h64, -2), (W, w64, -1)):
+            assert (size - crop) % 2 == 0, \
+                f"Can only handle even padding. Target_size={size}, Actual_size={crop} on dim {dim}."
+        return ((H - h64) // 2, (W - w64) // 2), (h64, w64)
+
+    def _run(self, st: dict) -> None:
+        """images (2,3,H,W) -> depth / var (1,1,H,W) inside the crop: crop, normalise, encoder, decoders, heads"""
+        (my, mx), (h64, w64) = st["margin"], st["crop"]
+        net, bf = self.net, st["bf"]
+        ims = (st["images"][:, :, my:my + h64, mx:mx + w64] - self._mean) / self._std
+        ctx, cats = net.encode(ims)
+        xd = net.decode(stereonet.DISP, ctx, cats)
+        xc = net.decode(stereonet.COV, ctx, cats) if self.est_cov else None
+        if st["kernel"]:
+            wd, sd_ = net.head[stereonet.DISP]
+            wc, sc = net.head[stereonet.COV] if self.est_cov else (None, None)
+            ops.stereo_head(xd, xc, cats[0], wd, sd_, wc, sc, bf, (my, mx), st["depth"], st["var"])
+            return
+        out_d = net.head_torch(stereonet.DISP, xd, cats[0])
+        out_c = net.head_torch(stereonet.COV, xc, cats[0]) if self.est_cov else None
+        depth, var = stereonet.depth_torch(out_d, out_c, bf)
+        st["depth"][..., my:my + h64, mx:mx + w64].copy_(depth)
+        if var is not None:
+            st["var"][..., my:my + h64, mx:mx + w64].copy_(var)
+
+    def _capture(self, run):
+        """capture `run` as a CUDA graph (after a warm-up run outside the capture, for cuDNN's algorithm choice); returns a
+        callable that replays it"""
+        side = torch.cuda.Stream(self.device)
+        side.wait_stream(torch.cuda.current_stream())
+        with torch.cuda.stream(side):
+            run()
+        torch.cuda.current_stream().wait_stream(side)
+        graph = torch.cuda.CUDAGraph()
+        n0 = ops.LAUNCHES[0]
+        with torch.cuda.graph(graph):
+            run()
+        launches = ops.LAUNCHES[0] - n0
+
+        def replay():
+            graph.replay()
+            ops.LAUNCHES[0] += launches
+        return replay
+
+    def estimate(self, frame: StereoData) -> IStereoDepth.Output:
+        with torch.inference_mode():
+            imgL, imgR = frame.imageL, frame.imageR
+            assert imgL.size(0) == 1 and imgR.size(0) == 1, "The interface will not handle batch dimension correctly."
+            H, W = imgL.shape[-2:]
+            assert tuple(imgR.shape[-2:]) == (H, W), "both images must have the same size"
+            bf = frame.frame_baseline * frame.fx
+            kernel = self.device.type == "cuda" and bool(torch.backends.cudnn.allow_tf32)
+            st = self._static
+            if self._replay is not None:
+                assert (H, W) == st["shape"], f"image shape changed since the CUDA graph was captured: {(H, W)} != {st['shape']}"
+                assert bf == st["bf"], "camera baseline * fx changed since the CUDA graph was captured"
+                if kernel != st["kernel"]:          # the TF32 flag changed: the other head path needs its own graph
+                    self._replay = None
+            if self._replay is None:
+                margin, crop = self.geometry(H, W)
+                nan = lambda: torch.full((1, 1, H, W), float("nan"), dtype=torch.float32, device=self.device)
+                st = self._static = {"shape": (H, W), "margin": margin, "crop": crop, "bf": bf, "kernel": kernel,
+                                     "images": torch.empty((2, 3, H, W), dtype=torch.float32, device=self.device),
+                                     "depth": nan(), "var": nan() if self.est_cov else None}
+            st["images"][0:1].copy_(imgL, non_blocking=True)
+            st["images"][1:2].copy_(imgR, non_blocking=True)
+            run = lambda: self._run(st)
+            # deterministic cuDNN algorithms (the transposed convolutions would otherwise be free to accumulate with atomics),
+            # so that a graph replay, the first call and cuda_graph: false give the same bits; TF32 and the other flags as
+            # they are
+            with torch.backends.cudnn.flags(enabled=torch.backends.cudnn.enabled, benchmark=torch.backends.cudnn.benchmark,
+                                            benchmark_limit=torch.backends.cudnn.benchmark_limit, deterministic=True,
+                                            allow_tf32=torch.backends.cudnn.allow_tf32):
+                if not self.use_graph:
+                    run()
+                elif self._replay is None:
+                    self._replay = self._capture(run)
+                    self._replay()
+                else:
+                    self._replay()
+            if self.est_cov:
+                return IStereoDepth.Output(depth=st["depth"].clone(), cov=st["var"].clone())
+            return IStereoDepth.Output(depth=st["depth"].clone())
+
+    @classmethod
+    def is_valid_config(cls, config: SimpleNamespace | None) -> None:
+        spec = {
+            "weight": lambda f: isinstance(f, str),
+            "device": lambda dev: isinstance(dev, str) and "cuda" in dev,
+            "cov_mode": lambda m: m in {"Est", "None"},
+        }
+        if config is not None and "cuda_graph" in vars(config):
+            spec["cuda_graph"] = lambda b: isinstance(b, bool)
+        cls._enforce_config_spec(config, spec)
+
+
 PLUGINS = {
     "frontend": B200_FlowFormerCovFrontend,
     "frontend_plain": B200_FlowFormerFrontend,
@@ -1154,4 +1303,5 @@ PLUGINS = {
     "optimizer": B200_TwoFrame_PGO,
     "motion": B200_TartanMotionNet,
     "matcher_tartanvo": B200_TartanVOMatcher,
+    "depth_tartanvo": B200_TartanVODepth,
 }
