@@ -220,11 +220,8 @@ flow_im2col_kernel(const float* __restrict__ coords1, const float* __restrict__ 
 template <int N>
 int launch_conv(const CUtensorMap& map_a, const CUtensorMap& map_w, const ConvArgs& a, int tiles, int slices, int smem_bytes,
                 cudaStream_t stream) {
-    static bool configured = false;
-    if (!configured) {
-        MACVO_CUDA_TRY(cudaFuncSetAttribute(conv_tc_kernel<N>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_MAX));
-        configured = true;
-    }
+    // the attribute belongs to the current device, so it is set on every launch (host-only, allowed under graph capture)
+    MACVO_CUDA_TRY(cudaFuncSetAttribute(conv_tc_kernel<N>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_MAX));
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3(tiles, slices);
     cfg.blockDim = dim3(TC_THREADS);

@@ -218,11 +218,8 @@ size_t operand_bytes(int batch, int dim, int n) { return ((size_t)batch * n * di
 template <int PASSES>
 int launch_main(const CUtensorMap& a_hi, const CUtensorMap& a_lo, const CUtensorMap& b_hi, const CUtensorMap& b_lo,
                 float* m_out, int batch, int n, int dim, int ctas, cudaStream_t st) {
-    static bool configured = false;
-    if (!configured) {
-        MACVO_CUDA_TRY(cudaFuncSetAttribute(corr_tc_kernel<PASSES>, cudaFuncAttributeMaxDynamicSharedMemorySize, CorrCfg<PASSES>::SMEM));
-        configured = true;
-    }
+    // the attribute belongs to the current device, so it is set on every launch (host-only, allowed under graph capture)
+    MACVO_CUDA_TRY(cudaFuncSetAttribute(corr_tc_kernel<PASSES>, cudaFuncAttributeMaxDynamicSharedMemorySize, CorrCfg<PASSES>::SMEM));
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3(ctas);
     cfg.blockDim = dim3(TC_THREADS);

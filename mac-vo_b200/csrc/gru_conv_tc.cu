@@ -258,11 +258,8 @@ bool make_map_a(CUtensorMap* map, const void* base, int channels, const Geometry
 template <int STAGE>
 int launch_stage(const CUtensorMap* maps, Unit u, const Geometry& g, cudaStream_t stream) {
     constexpr int N = STAGE == 0 ? 256 : 128;
-    static bool configured = false;
-    if (!configured) {
-        MACVO_CUDA_TRY(cudaFuncSetAttribute(gru_conv_tc_kernel<STAGE>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<N>::SMEM));
-        configured = true;
-    }
+    // the attribute belongs to the current device, so it is set on every launch (host-only, allowed under graph capture)
+    MACVO_CUDA_TRY(cudaFuncSetAttribute(gru_conv_tc_kernel<STAGE>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<N>::SMEM));
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3(g.tiles);
     cfg.blockDim = dim3(TC_THREADS);

@@ -224,11 +224,8 @@ int macvo_mlp_tc(const float* xn, const float* resid, const float* w1, const flo
     ok = ok && make_map_2d(&m_w1, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, w1, MLP_C, hidden, MLP_C * 4, 32, MLP_CHUNK);
     ok = ok && make_map_2d(&m_w2, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, w2, hidden, MLP_C, (uint64_t)hidden * 4, 32, MLP_C);
     if (!ok) return MACVO_E_DRIVER;
-    static bool configured = false;
-    if (!configured) {
-        MACVO_CUDA_TRY(cudaFuncSetAttribute(mlp_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, MLP_SMEM));
-        configured = true;
-    }
+    // the attribute belongs to the current device, so it is set on every launch (host-only, allowed under graph capture)
+    MACVO_CUDA_TRY(cudaFuncSetAttribute(mlp_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, MLP_SMEM));
     mlp_tc_kernel<<<ceil_div(rows, MLP_ROWS), MLP_THREADS, MLP_SMEM, as_stream(stream)>>>(m_x, m_w1, m_w2, b1, b2, resid, out,
                                                                                           rows, hidden);
     MACVO_LAUNCH_CHECK();

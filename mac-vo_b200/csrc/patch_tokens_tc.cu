@@ -213,14 +213,11 @@ int macvo_patch_tokens_tc(const float* x, const float* w0, const float* term, co
     ok = ok && make_map_2d(&m_w0, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, w0, PT_IN, PT_C, PT_IN * 4, 32, PT_C);
     ok = ok && make_map_2d(&m_w2, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, w2, PT_C, PT_C, PT_C * 4, 32, PT_C);
     if (!ok) return MACVO_E_DRIVER;
-    static int sms = 0;
-    if (!sms) {
-        int dev = 0, n = 0;
-        MACVO_CUDA_TRY(cudaGetDevice(&dev));
-        MACVO_CUDA_TRY(cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev));
-        MACVO_CUDA_TRY(cudaFuncSetAttribute(patch_tokens_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, PT_SMEM));
-        sms = n;
-    }
+    // the SM count and the attribute belong to the current device: both are taken on every launch (host-only calls)
+    int dev = 0, sms = 0;
+    MACVO_CUDA_TRY(cudaGetDevice(&dev));
+    MACVO_CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    MACVO_CUDA_TRY(cudaFuncSetAttribute(patch_tokens_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, PT_SMEM));
     const int tiles = ceil_div((int)rows, PT_ROWS);
     patch_tokens_tc_kernel<<<tiles < sms ? tiles : sms, TC_THREADS, PT_SMEM, as_stream(stream)>>>(
         m_x, m_w0, m_w2, term, b2, ln_w, ln_b, out, (int)rows, period, eps);

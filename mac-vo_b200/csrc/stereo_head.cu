@@ -194,11 +194,8 @@ int macvo_stereo_head(const float* xd, const float* xc, const float* cat0, int h
     if ((long long)margin_y + 2LL * h2 > height || (long long)margin_x + 2LL * w2 > width) return MACVO_E_ARG;
     for (const void* p : {(const void*)w11_d, (const void*)w11_c})
         if (reinterpret_cast<uintptr_t>(p) & 15) return MACVO_E_ARG;
-    static bool attr = false;
-    if (!attr) {
-        MACVO_CUDA_TRY(cudaFuncSetAttribute(stereo_head_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SH_SMEM));
-        attr = true;
-    }
+    // the attribute belongs to the current device, so it is set on every launch (host-only, allowed under graph capture)
+    MACVO_CUDA_TRY(cudaFuncSetAttribute(stereo_head_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SH_SMEM));
     const dim3 grid(ceil_div(w2, SH_TILE), ceil_div(h2, SH_TILE));
     stereo_head_kernel<<<grid, SH_THREADS, SH_SMEM, as_stream(stream)>>>(xd, xc, cat0, h2, w2, w11_d, small_d, w11_c,
                                                                         small_c, bf, bf2, margin_y, margin_x, height,

@@ -17,6 +17,7 @@ from oracle import frontend as ofe
 from oracle import keypoint as okp
 from oracle import pgo as opgo
 from tests.golden import cases
+from tests.kernel_inventory import expect_variants
 
 pytestmark = pytest.mark.gpu
 
@@ -73,8 +74,8 @@ def test_corr_tensor_core_3xf16(ops, shape):
         with pytest.raises(ops.MacvoB200Error):
             ops.corr_build(f1.to(DEV), f2.to(DEV), mode=ops.CORR_TC_3XF16)
         return
-    out = ops.corr_build(f1.to(DEV), f2.to(DEV), mode=ops.CORR_TC_3XF16)
-    torch.cuda.synchronize()
+    d1, d2 = f1.to(DEV), f2.to(DEV)
+    out = expect_variants(lambda: ops.corr_build(d1, d2, mode=ops.CORR_TC_3XF16), "corr_tc_kernel<3>", "split_transpose_kernel")
     _corr_check(out, f1, f2, 2e-6)
     simt = ops.corr_build(f1.to(DEV), f2.to(DEV), mode=ops.CORR_SIMT)
     torch.testing.assert_close(out, simt, rtol=1e-4, atol=2e-4)
@@ -97,8 +98,7 @@ def test_corr_tensor_core_tf32(ops, shape, layout):
         with pytest.raises(ops.MacvoB200Error):
             ops.corr_build(d1, d2, mode=ops.CORR_TC_TF32)
         return
-    out = ops.corr_build(d1, d2, mode=ops.CORR_TC_TF32)
-    torch.cuda.synchronize()
+    out = expect_variants(lambda: ops.corr_build(d1, d2, mode=ops.CORR_TC_TF32), "corr_tc_kernel<2>")
     n = H1 * W1
     if n <= 6400:
         _corr_check(out, f1, f2, 6e-4)
@@ -133,7 +133,8 @@ def test_corr_tensor_core_1xf16_exact_for_fp16_features(ops):
     """MACVO_Fast: features are already fp16 -> one tensor-core pass is exact (fp32 accumulate)."""
     f1, f2 = cases.corr_inputs(2, 30, 40)
     f1h, f2h = f1.half(), f2.half()
-    out = ops.corr_build(f1h.to(DEV), f2h.to(DEV))                   # dispatches to the 1-pass mode
+    d1, d2 = f1h.to(DEV), f2h.to(DEV)
+    out = expect_variants(lambda: ops.corr_build(d1, d2), "corr_tc_kernel<1>")     # dispatches to the 1-pass mode
     _corr_check(out, f1h.float(), f2h.float(), 5e-7)
 
 
@@ -227,11 +228,11 @@ def test_selectors_bit_exact(ops, golden, name):
     d = ops.dense_postproc(flow.to(DEV), cov.to(DEV), 0.25 * 320.0, False, score=score)   # fused scoring
     cand = ops.CandidateList(H, W, DEV)
     mm = cases.selector_match_mask(H, W).to(DEV) if g["variant"] == "masked" else None
-    ops.select_candidates(score, 32, 100.0, mm, cand)
+    expect_variants(lambda: ops.select_candidates(score, 32, 100.0, mm, cand), "flag_count_kernel<0>")
     torch.manual_seed(cases.SELECTOR_RNG_SEED)
     kp = ops.sample_candidates(cand, g["num"])
     mcand = ops.CandidateList(H, W, DEV)
-    ops.select_mapping_candidates(d["depth"], d["depth_cov"], 32, 5.0, 0.005, mcand)
+    expect_variants(lambda: ops.select_mapping_candidates(d["depth"], d["depth_cov"], 32, 5.0, 0.005, mcand), "flag_count_kernel<1>")
     mp = ops.sample_candidates(mcand, 2000)
     assert kp.dtype == torch.int64 and kp.is_cuda
     assert torch.equal(kp.cpu(), g["kp"]), "keypoint indices must be bit-exact"
@@ -281,7 +282,8 @@ def test_depth_aware_selector_bit_exact(ops, golden, name):
     mm = cases.selector_match_mask(H, W).to(DEV) if g["variant"] == "masked" else None
     score, cand = ops.ScoreBuffers(H, W, DEV, 7), ops.CandidateList(H, W, DEV)
     ops.score_depth_aware(d1["flow_cov"], d0["depth_cov"], d1["depth_cov"], score)
-    ops.select_candidates_depth(score, d0["depth"], d1["depth"], d0["depth_cov"], 32, 320.0 * 0.25, 250.0, 100.0, m0, mm, cand)
+    expect_variants(lambda: ops.select_candidates_depth(score, d0["depth"], d1["depth"], d0["depth_cov"], 32, 320.0 * 0.25, 250.0,
+                                                        100.0, m0, mm, cand), "flag_count_kernel<2>")
     torch.manual_seed(cases.SELECTOR_RNG_SEED)
     kp = ops.sample_candidates(cand, g["num"])
     assert torch.equal(kp.cpu(), g["kp"]), "depth-aware keypoint indices must be bit-exact"
@@ -293,8 +295,10 @@ def test_retrieve_pixels(ops):
     m = torch.randn(1, 3, 50, 70, generator=g)
     kp_i = torch.stack([torch.randint(0, 70, (40,), generator=g), torch.randint(0, 50, (40,), generator=g)], -1)
     kp_f = kp_i.float() + torch.rand(40, 2, generator=g) * 0.99
-    for kp in (kp_i, kp_f):
-        out = ops.retrieve_pixels(kp.to(DEV), m.to(DEV)).cpu()
+    dm = m.to(DEV)
+    for kp, variant in ((kp_i, "retrieve_pixels_kernel<long>"), (kp_f, "retrieve_pixels_kernel<float>")):
+        dkp = kp.to(DEV)
+        out = expect_variants(lambda: ops.retrieve_pixels(dkp, dm), variant).cpu()
         assert torch.equal(out, ofe.retrieve_pixels(kp, m))
 
 
@@ -305,7 +309,9 @@ def test_match_covariance(ops, golden, name):
     H, W, K = g["shape"]
     kp, depth, flow_cov = cases.cov_inputs(H, W, K, g["kind"])
     fc = None if flow_cov is None else flow_cov.to(DEV)
-    cov, pt, status = ops.match_covariance(kp.to(DEV), depth.to(DEV), fc, 320.0, 320.0, W / 2, H / 2, want_point=True)
+    dkp, dd = kp.to(DEV), depth.to(DEV)
+    variant = "match_cov_kernel<long>" if kp.dtype == torch.int64 else "match_cov_kernel<float>"
+    cov, pt, status = expect_variants(lambda: ops.match_covariance(dkp, dd, fc, 320.0, 320.0, W / 2, H / 2, want_point=True), variant)
     assert cov.dtype == torch.float64 and cov.shape == (K, 3, 3) and int(status.item()) == 0
     # 1e-5 relative to each matrix' scale (north_star tolerance: 1e-4)
     ref = g["out"]
@@ -361,11 +367,12 @@ def test_pgo_solve_large(ops, K):
     c = cases.pgo_inputs(K, 6)
     ref = opgo.lm_solve(cases.pgo_graph(c))
     poses = []
-    for cluster in (1, 8):
+    for cluster in (1, 3, 5, 6, 7, 8):
         pose, _ = ops.pgo_solve(*_pgo_device_args(c), cluster=cluster)
         poses.append(pose.cpu().numpy())
         np.testing.assert_allclose(poses[-1], ref, rtol=1e-8, atol=1e-9)
-    np.testing.assert_allclose(poses[0], poses[1], rtol=1e-12, atol=1e-13)
+    for p in poses[1:]:
+        np.testing.assert_allclose(p, poses[0], rtol=1e-12, atol=1e-13)
 
 
 def test_pgo_accumulate_packed(ops):
@@ -389,8 +396,8 @@ def test_corr_build_channels_last_inputs_bit_identical(ops):
     """K-major (channels_last) features take the elementwise operand split; same operands -> same bits as the NCHW path"""
     f1, f2 = cases.corr_inputs(2, 12, 16)
     a = ops.corr_build(f1.to(DEV), f2.to(DEV))
-    b = ops.corr_build(f1.to(DEV).contiguous(memory_format=torch.channels_last),
-                       f2.to(DEV).contiguous(memory_format=torch.channels_last))
+    c1, c2 = (t.to(DEV).contiguous(memory_format=torch.channels_last) for t in (f1, f2))
+    b = expect_variants(lambda: ops.corr_build(c1, c2), "corr_tc_kernel<3>", "split_kmajor_kernel")
     assert torch.equal(a, b)
     c = ops.corr_build(f1.to(DEV).contiguous(memory_format=torch.channels_last),
                        f2.to(DEV).contiguous(memory_format=torch.channels_last), mode=ops.CORR_TC_1XF16)
@@ -507,7 +514,7 @@ def test_pgo_other_graph_types(ops, golden, name):
     inp = P.PGOInput(pos_Tw=c["pos_Tw"], kp2_uv=c["kp2_uv"], kp2_disp=c["kp2_disp"], uv_cov=c["uv_cov"], disp_cov=c["disp_cov"],
                      K=c["K"], baseline=c["baseline"], init_pose=c["init_pose"], kp2_d=c["kp2_d"], obs_cov=c["obs_cov"],
                      pts_cov=c["pts_cov"])
-    for cluster in (1, 2):
+    for cluster in (1, 2, 3, 5, 6, 7):
         pose, stats = P.solve_two_frame_pgo(inp, DEV, cluster, g["graph_type"])
         np.testing.assert_allclose(pose.cpu().numpy(), ref, rtol=1e-8, atol=1e-9)
         np.testing.assert_allclose(pose.cpu().numpy(), g["pose"].double().numpy(), rtol=1e-8, atol=1e-9)

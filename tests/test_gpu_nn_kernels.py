@@ -5,6 +5,8 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+from tests.kernel_inventory import expect_variants
+
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
 
@@ -18,6 +20,9 @@ def ops():
     return ops
 
 
+LAYER_NORM_VARIANT = {64: "layer_norm64_kernel", 128: "layer_norm_kernel<4>", 256: "layer_norm_kernel<8>", 512: "layer_norm_kernel<16>"}
+
+
 @pytest.mark.parametrize("rows,c", [(1, 128), (7, 128), (4801, 128), (300, 256), (65, 512), (9600 * 8, 128), (9601, 64)])
 def test_layer_norm(ops, rows, c):
     g = torch.Generator().manual_seed(rows + c)
@@ -25,7 +30,7 @@ def test_layer_norm(ops, rows, c):
     w, b = torch.randn(c, generator=g).to(DEV), torch.randn(c, generator=g).to(DEV)
     for eps in (1e-5, 1e-6):
         ref = F.layer_norm(x.double(), (c,), w.double(), b.double(), eps)
-        got = ops.layer_norm(x, w, b, eps)
+        got = expect_variants(lambda: ops.layer_norm(x, w, b, eps), LAYER_NORM_VARIANT[c])
         assert (got.double() - ref).abs().max().item() <= 1e-5 * ref.abs().max().item()
     with pytest.raises(ops.MacvoB200Error):
         ops.layer_norm(x[:, :32].contiguous(), w[:32], b[:32])
@@ -72,6 +77,16 @@ ATTN_CASES = [(37, 8, 80, 8, 16, True), (50, 8, 8, 8, 16, False), (33, 1, 8, 8, 
               (41, 1, 8, 8, 8, False), (6, 8, 20, 8, 8, True), (77, 1, 8, 4, 16, False), (300, 1, 5, 8, 8, False)]
 
 
+def _attn_variant(b, nq, heads, d, bc, tf32):
+    """macvo_small_attention_ex's choice for plain (B, N, C) operands (csrc/nn_kernels.cu): one query, up to 8 queries of 8
+    heads (4 slots x 2), the tensor-core kernel for 16+ queries in TF32 mode, else the shared-K/V kernel"""
+    if nq == 1 and not bc and d <= 16:
+        return f"attn_single_query_kernel<{d}>"
+    if nq <= 8 and heads == 8 and d <= 16:
+        return f"attn_few_queries_kernel<{d}>"
+    return f"attn_tc_kernel<{d}>" if tf32 and nq >= 16 else f"attn_shared_kv_kernel<{d}>"
+
+
 @pytest.mark.parametrize("case", ATTN_CASES)
 def test_small_attention(ops, case):
     b, nq, nk, heads, d, bc = case
@@ -80,11 +95,11 @@ def test_small_attention(ops, case):
     k = (torch.randn(b, nk, heads * d, generator=g) * 1.5).to(DEV)
     v = torch.randn(b, nk, heads * d, generator=g).to(DEV)
     ref = _ref_attention(q, k, v, heads)
-    got = ops.small_attention(q, k, v, heads, allow_tf32=False)
+    got = expect_variants(lambda: ops.small_attention(q, k, v, heads, allow_tf32=False), _attn_variant(b, nq, heads, d, bc, False))
     assert got.shape == ref.shape
     assert (got.double() - ref).abs().max().item() <= 2e-5 * ref.abs().max().item()
     # tensor-core path (TF32 operands, fp32 accumulate): the tolerance of a TF32 bmm-softmax-bmm
-    got = ops.small_attention(q, k, v, heads, allow_tf32=True)
+    got = expect_variants(lambda: ops.small_attention(q, k, v, heads, allow_tf32=True), _attn_variant(b, nq, heads, d, bc, True))
     assert (got.double() - ref).abs().max().item() <= 4e-3 * ref.abs().max().item()
 
 
@@ -163,6 +178,13 @@ def test_sepconv_gru_wgmma(ops, shape):
             h = (1 - z) * h + z * q
         return h
 
+    # launch probe on a throwaway step, then back to the initial state (set_state rebuilds every operand a step reads):
+    # every step runs both stages, the z / r convolution and then the q convolution
+    zeros = torch.zeros(P, 128, device=DEV)
+    expect_variants(lambda: torch.cuda.current_stream().wait_event(gru.step(zeros, zeros, gamma)), "gru_conv_tc_kernel<0>",
+                    "gru_conv_tc_kernel<1>", "pack_motion_kernel")
+    for u in range(2):
+        gru.set_state(u, h0[u])
     ref_r, ref_t = [to_map(h) for h in h0], [to_map(h) for h in h0]
     for it in range(2):
         mf, agg = rnd(P, 128).relu(), rnd(P, 128)
@@ -235,6 +257,21 @@ def _from_rows_u(rows, shape):
     return body[:, 2:H + 2, 2:W + 2].permute(0, 3, 1, 2).double()
 
 
+def _conv_tiles(b, h, w):
+    """128-row tiles over the layout-U padded pixels of a (b, h, w) map"""
+    return -(-(b * (h + 4) * (w + 4)) // 128)
+
+
+def _conv_n_cta(n_pad, tiles, sms):
+    """macvo_conv_tc's output-channel slicing (csrc/conv_tc.cu): as many slices as fit one wave of CTAs, each a multiple of 32
+    columns and at most 256 wide (a wider single slice forces the slicing past one wave)"""
+    slices = 1
+    for s in range(1, 9):
+        if n_pad % (32 * s) == 0 and n_pad // s <= 256 and (tiles * s <= sms or n_pad // slices > 256):
+            slices = s
+    return n_pad // slices
+
+
 @pytest.mark.parametrize("shape", [(1, 60, 80), (2, 13, 17), (1, 90, 160)])
 @pytest.mark.parametrize("cin,cout,k,relu", [(256, 192, 3, True), (128, 256, 3, True), (256, 2, 3, False), (192, 256, 1, True),
                                              (128, 126, 3, True), (64, 2, 3, False), (128, 64, 3, True)])
@@ -256,7 +293,9 @@ def test_conv_tc(ops, shape, cin, cout, k, relu):
     out16 = torch.zeros(ops.rows_count(B, H, W), 256, dtype=torch.float16, device=DEV)
     o32 = 4 if H % 2 == 0 else 1                                # vector-store path | scalar path
     out32 = torch.full((P, cout + 8), 7.0, device=DEV)
-    ops.conv_tc(rows, wp, bp, n, k, relu, shape, out16=out16, out16_offset=64 if cout <= 192 else 0, out32=out32, out32_offset=o32)
+    n_cta = _conv_n_cta(wp.shape[0], _conv_tiles(B, H, W), torch.cuda.get_device_properties(0).multi_processor_count)
+    expect_variants(lambda: ops.conv_tc(rows, wp, bp, n, k, relu, shape, out16=out16, out16_offset=64 if cout <= 192 else 0,
+                                        out32=out32, out32_offset=o32), f"conv_tc_kernel<{n_cta}>")
     got32 = out32[:, o32:o32 + cout].view(B, H, W, cout).permute(0, 3, 1, 2).double()
     assert (got32 - ref).abs().max().item() <= 1e-3 * scale
     assert (out32[:, :o32] == 7.0).all() and (out32[:, o32 + cout:] == 7.0).all()                   # neighbours untouched
@@ -277,6 +316,63 @@ def test_conv_tc(ops, shape, cin, cout, k, relu):
         assert (o16.view(B, H, W, cout).permute(0, 3, 1, 2).double() - ref2).abs().max().item() <= 2e-3 * ref2.abs().max().item()
     with pytest.raises(ops.MacvoB200Error):
         ops.conv_tc(rows[:-1], wp, bp, n, k, relu, shape, out32=out32)
+
+
+@pytest.mark.parametrize("k", [1, 3])
+@pytest.mark.parametrize("cout,n_cta", [(192, 96), (150, 160), (224, 224), (320, 160)])
+def test_conv_tc_slice_widths(ops, cout, n_cta, k):
+    """the slice widths only some shapes select: 96 columns (a 7-slot operand ring), 160 (5 slots; cout 150 also leaves 10
+    padded columns unstored), 224 (4 slots), and cout 320, which is cut into two 160-column slices even when that takes more
+    than one wave. The width W is chosen from the SM count S with a copy of macvo_conv_tc's rule; the probe proves the choice.
+    Enough K steps (64-channel blocks x taps) for the ring to wrap: 18 for 3x3 over 128 channels, 8 for 1x1 over 512.
+    float64 reference on the fp16-rounded operands: 1e-3 (fp32 rows) / 2e-3 (fp16 rows) of the output scale."""
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    n_pad = -(-cout // 32) * 32
+    if cout == 320:
+        B, H, W = 1, 90, 160
+        assert 2 * _conv_tiles(B, H, W) > sms                   # two slices are more than one wave: the 256-column limit forces them
+    else:
+        B, H = 1, 60
+        W = next(w for w in range(60, 400) if _conv_n_cta(n_pad, _conv_tiles(B, H, w), sms) == n_cta)
+    tiles = _conv_tiles(B, H, W)
+    assert _conv_n_cta(n_pad, tiles, sms) == n_cta
+    print(f"conv_tc: S = {sms}, {B} x {H} x {W}, cout {cout} (n_pad {n_pad}), {tiles} tiles -> {n_pad // n_cta} slices of {n_cta}")
+    shape, P, cin, relu = (B, H, W), B * H * W, (128 if k == 3 else 512), k == 3
+    g = torch.Generator().manual_seed(cout * 10 + k)
+    x = torch.randn(B, cin, H, W, generator=g).to(DEV)
+    w = (torch.randn(cout, cin, k, k, generator=g) * (cin * k * k) ** -0.5).to(DEV)
+    b = torch.randn(cout, generator=g).to(DEV)
+    ref = F.conv2d(x.half().double(), w.half().double(), b.double(), padding=k // 2)
+    if relu:
+        ref = ref.relu()
+    scale = ref.abs().max().item()
+    wp, bp, n = ops.pack_conv_filter(w, b)
+    rows = _to_rows_u(ops, x, shape)
+    out16 = torch.zeros(ops.rows_count(B, H, W), n_pad, dtype=torch.float16, device=DEV)
+    out32 = torch.full((P, cout), 7.0, device=DEV)
+    expect_variants(lambda: ops.conv_tc(rows, wp, bp, n, k, relu, shape, out16=out16, out32=out32), f"conv_tc_kernel<{n_cta}>")
+    got32 = out32.view(B, H, W, cout).permute(0, 3, 1, 2).double()
+    assert (got32 - ref).abs().max().item() <= 1e-3 * scale
+    got16 = _from_rows_u(out16, shape)
+    assert (got16[:, :cout] - ref).abs().max().item() <= 2e-3 * scale
+    assert not got16[:, cout:].any()                                 # padded filter columns are never stored
+
+
+def test_conv_tc_rejects_unsliceable_width(ops):
+    """352 output columns: no slice width (a multiple of 32, at most 256) divides them, so the call is refused and writes nothing"""
+    B, H, W = 1, 12, 16
+    shape, P = (B, H, W), B * H * W
+    g = torch.Generator().manual_seed(352)
+    x = torch.randn(B, 64, H, W, generator=g).to(DEV)
+    wp, bp, n = ops.pack_conv_filter((torch.randn(352, 64, 3, 3, generator=g) * 0.05).to(DEV), torch.randn(352, generator=g).to(DEV))
+    assert wp.shape[0] == 352
+    rows = _to_rows_u(ops, x, shape)
+    out16 = torch.full((ops.rows_count(B, H, W), 352), 3.0, dtype=torch.float16, device=DEV)
+    out32 = torch.full((P, 352), 7.0, device=DEV)
+    with pytest.raises(ops.MacvoB200Error):
+        ops.conv_tc(rows, wp, bp, n, 3, True, shape, out16=out16, out32=out32)
+    torch.cuda.synchronize()
+    assert (out16 == 3.0).all() and (out32 == 7.0).all()
 
 
 def test_flow_im2col(ops):
@@ -306,8 +402,9 @@ def test_lookup_rows_equals_lookup_map(ops):
     sys.path.insert(0, os.path.join(os.path.dirname(__file__), "golden"))
     import cases
     cm, co = cases.lookup_inputs(2, 12, 16)
-    a = ops.corr_lookup(cm.to(DEV), co.to(DEV))
-    b = ops.corr_lookup(cm.to(DEV), co.to(DEV), rows=True)
+    cm, co = cm.to(DEV), co.to(DEV)
+    a = expect_variants(lambda: ops.corr_lookup(cm, co), "corr_lookup_kernel<false>")
+    b = expect_variants(lambda: ops.corr_lookup(cm, co, rows=True), "corr_lookup_kernel<true>")
     assert b.shape == (2 * 12 * 16, 81)
     assert torch.equal(a.permute(0, 2, 3, 1).reshape(-1, 81), b)          # same arithmetic, other layout: bit-exact
 
@@ -348,25 +445,41 @@ def test_latent_pool_equals_cross_attention(ops, m, nk):
     assert (got.double() - ref).abs().max().item() <= 4e-3 * ref.abs().max().item()
 
 
-@pytest.mark.parametrize("b,h,w", [(1, 5, 7), (2, 12, 16), (2, 60, 80), (1, 33, 47)])
+def _token_tile(pixels, sms):
+    """macvo_decoder_token's tile choice (csrc/decoder_token.cu): 72-pixel tiles when, at one CTA per SM, they need fewer
+    pixel slots over all waves than 64-pixel tiles"""
+    cost = lambda tp: -(-(-(-pixels // tp)) // sms) * tp
+    return 72 if cost(72) < cost(64) else 64
+
+
+# the last case takes its width from the SM count S: a pixel count in (64 S, 72 S] selects 72-pixel tiles
+@pytest.mark.parametrize("b,h,w", [(1, 5, 7), (2, 12, 16), (2, 60, 80), (1, 33, 47), pytest.param(2, 55, None, id="tile72")])
 def test_decoder_token_kernel(ops, b, h, w):
     """csrc/decoder_token.cu vs a float64 torch evaluation of the chain it replaces (decoder.py:20-76,112-116) with the
     network's own weights: token MLP, LayerNorm + sine embedding, q projection, 8-head attention over the pixel's 8
-    cost-memory tokens, output projection, FFN; out = [cost_global | cost_forward | 0]. fp32 FMA kernel -> 1e-5."""
+    cost-memory tokens, output projection, FFN; out = [cost_global | cost_forward | 0]. fp32 FMA kernel -> 1e-5.
+    Both tile widths run, each with fp32 rows and fp16 layout-U rows out; the 72-pixel case has a ragged last tile and the
+    batch boundary inside a tile."""
     from macvo_b200.flowformer_cov import synthetic_state_dict, sine_embed
     sd = {k: v.to(DEV) for k, v in synthetic_state_dict(0).items() if k.startswith("memory_decoder.")}
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    if w is None:
+        w = next(w for w in range(1, 4096) if _token_tile(b * h * w, sms) == 72 and (b * h * w) % 72 and (h * w) % 72)
     P = b * h * w
+    tile = _token_tile(P, sms)
+    print(f"decoder_token: S = {sms}, B x H x W = {b} x {h} x {w} = {P} pixels -> {tile}-pixel tiles")
     g = torch.Generator().manual_seed(P)
     cf = torch.randn(P, 81, generator=g).to(DEV) * 2
     ys, xs = torch.meshgrid(torch.arange(h, dtype=torch.float32), torch.arange(w, dtype=torch.float32), indexing="ij")
     coords = (torch.stack([xs, ys], 0).unsqueeze(0).repeat(b, 1, 1, 1) + torch.randn(b, 2, h, w, generator=g) * 5).to(DEV)
     key, value = torch.randn(P, 8, 64, generator=g).to(DEV), torch.randn(P, 8, 64, generator=g).to(DEV)
     blob = ops.decoder_token_blob(sd)
-    got = ops.decoder_token(cf, coords, key, value, blob)
+    variant = f"decoder_token_kernel<{tile}>"
+    got = expect_variants(lambda: ops.decoder_token(cf, coords, key, value, blob), variant)
     assert got.shape == (P, 160) and torch.equal(got[:, 64:145], cf) and not got[:, 145:].any()
     # the fp16 layout-U variant (the tensor-core motion encoder's input) holds the same rows, rounded once
     rows16 = torch.zeros(ops.rows_count(b, h, w), 192, dtype=torch.float16, device=DEV)
-    assert ops.decoder_token(cf, coords, key, value, blob, out16_rows=rows16) is rows16
+    assert expect_variants(lambda: ops.decoder_token(cf, coords, key, value, blob, out16_rows=rows16), variant) is rows16
     body = _from_rows_u(rows16, (b, h, w))                                      # (B, 192, H, W); asserts the padding stayed zero
     assert torch.equal(body[:, :160].permute(0, 2, 3, 1).reshape(P, 160), got.half().double()) and not body[:, 160:].any()
 
