@@ -16,6 +16,7 @@ provide the same names, signatures and error behaviour for the methods the hot p
     IMotionModel         Module/MotionModel.py:15-41
     IOptimizer           Module/Optimization/Interface.py:40-242 (sequential mode only)
     StereoData           DataLoader/Interface.py:57-113
+    StereoFrame          DataLoader/Interface.py:168-195
     ConfigTestable._enforce_config_spec  Utility/Extensions/Testable.py:23-42
 """
 from __future__ import annotations
@@ -117,6 +118,20 @@ class StereoData:
     def cx(self) -> float: return self.K[0, 0, 2].item()
     @property
     def cy(self) -> float: return self.K[0, 1, 2].item()
+
+
+@dataclass(kw_only=True)
+class StereoFrame:
+    """DataLoader/Interface.py:168-195 (DataFrame + StereoFrame): what a per-frame odometry driver reads"""
+    idx: list
+    time_ns: list
+    stereo: StereoData
+    gt_pose: object = None
+
+    @property
+    def frame_idx(self) -> int:
+        assert len(self.idx) == 1, "frame_idx property is only valid on unbatched data"
+        return self.idx[0]
 
 
 class IStereoDepth(ABC, _Registry):

@@ -453,3 +453,206 @@ class FusedTwoFrameOdometry:
             self._tail_done.synchronize()
         torch.cuda.current_stream().synchronize()
         return torch.stack([p.cpu().float() for p in self.pose_dev])
+
+
+def _deterministic_cudnn():
+    """the flags B200_TartanVOMatcher / B200_TartanVODepth run their networks under: deterministic cuDNN algorithms, every
+    other flag (TF32 included) as the caller set it"""
+    cudnn = torch.backends.cudnn
+    return cudnn.flags(enabled=cudnn.enabled, benchmark=cudnn.benchmark, benchmark_limit=cudnn.benchmark_limit,
+                       deterministic=True, allow_tf32=cudnn.allow_tf32)
+
+
+class FusedTartanVO:
+    """The data flow of the TartanVO baseline's driver (Odometry/BaselineTartanVO.py:35-60) on the device, built from the
+    three B200 plugins: `matcher` (B200_TartanVOMatcher), `depth` (B200_TartanVODepth with cov_mode "None": the covariance
+    decoder the baseline discards is not run) and `motion` (B200_TartanMotionNet). Their networks run as the plugins run
+    them (`_run`, `net.body`, `head`), into buffers this driver owns.
+
+    A frame is a keyframe when frame.frame_idx % keyframe_freq == 0 (UniformKeyframe; 1 for AllKeyframe). A non-keyframe
+    enqueues nothing: it carries the previous frame's pose and T_BS, with need_interp True. Per keyframe after the first:
+      * L(t) and R(t) cross PCIe once (from the frame's pinned memory, else through double-buffered pinned staging);
+        L(t-1) stays on the device from the previous keyframe;
+      * PWC-Net on (L(t-1), L(t)) on a side stream, next to the depth network on (L(t), R(t)) on the current stream;
+      * after the join, the pose network up to fc1 and its head on the previous pose, which stays on the device: an fp32
+        (7,) pose widened to float64 for the head and rounded back, exactly as B200_TartanMotionNet.predict carries it;
+      * the pose is written into a device-side trajectory.
+    The first keyframe gets the identity; its depth, which the baseline computes and never reads, is not computed.
+
+    cuda_graph (default True): a keyframe's work (both branches, the pose network and its head) is one CUDA graph, captured
+    at the second keyframe under the flags the plugins use and replayed after; the image shape, intrinsics and
+    baseline * fx must then stay the same. cuda_graph=False runs the same work eagerly.
+
+    Nothing in `run` waits on the device (`host_waits` records, per frame, whether the host had to wait for a staging
+    buffer, which only happens for frames in pageable memory), so frame t+1's networks are enqueued while frame t's still
+    run. `finish()` synchronises once and returns the (F, 7) fp32 poses and the (F,) need_interp flags; `frames` holds
+    what the map stores per frame (K, baseline, T_BS, time_ns)."""
+
+    def __init__(self, matcher, depth, motion, keyframe_freq: int = 1, cuda_graph: bool = True):
+        if depth.est_cov:
+            raise ValueError("FusedTartanVO runs the depth network without its covariance decoder: build "
+                             "B200_TartanVODepth with cov_mode 'None'")
+        if not (isinstance(keyframe_freq, int) and keyframe_freq >= 1):
+            raise ValueError(f"keyframe_freq must be an integer >= 1, got {keyframe_freq!r}")
+        from . import ops
+        self.ops = ops
+        self.matcher, self.depth, self.motion = matcher, depth, motion
+        self.device = motion.device
+        self.keyframe_freq, self.cuda_graph = keyframe_freq, cuda_graph
+        self.side = torch.cuda.Stream(self.device)
+        self.host_waits: list[int] = []
+        self.frames: list[dict] = []        # per frame: K, baseline, T_BS, time_ns, need_interp, row (of the trajectory)
+        self.traj = torch.empty((256, 7), dtype=torch.float32, device=self.device)    # one row per keyframe, grows x2
+        self.num_keyframes = 0
+        self._st: dict | None = None
+        self._graph = None
+        self._staging = None                # two pinned (2,3,H,W) buffers, for frames in pageable memory
+        self._staged = [None, None]         # the event after each staging buffer's upload
+
+    def _setup(self, stereo, H: int, W: int) -> None:
+        """static buffers for one image shape and camera"""
+        from . import posenet
+        dev, ops = self.device, self.ops
+        meta, K, bl_fx = self.motion._camera(stereo)
+        mmargin, mcrop = self.matcher.geometry(H, W)
+        dmargin, dcrop = self.depth.geometry(H, W)
+        nan = lambda c: torch.full((1, c, H, W), float("nan"), dtype=torch.float32, device=dev)
+        inp = torch.empty((1, 5, ops.POSENET_H, ops.POSENET_W), dtype=torch.float32, device=dev)
+        inp[:, 3:5] = posenet.intrinsic_layer(meta.height, meta.width, *K[:2], *K[2:], dev)
+        dimg = torch.empty((2, 3, H, W), dtype=torch.float32, device=dev)          # [L(t), R(t)]
+        self._st = {
+            "shape": (H, W), "K": K, "bl_fx": bl_fx, "dimg": dimg,
+            "mimg": torch.empty((2, 3, H, W), dtype=torch.float32, device=dev),    # [L(t-1), L(t)]
+            "mmargin": mmargin, "mcrop": mcrop, "flow": nan(2), "inp": inp,
+            "dst": {"margin": dmargin, "crop": dcrop, "bf": bl_fx, "kernel": None, "images": dimg, "depth": nan(1),
+                    "var": None},
+            "prev": torch.empty((7,), dtype=torch.float64, device=dev),             # the previous pose, widened
+            "next": torch.empty((7,), dtype=torch.float64, device=dev),             # the head's output
+            "pose": torch.empty((7,), dtype=torch.float32, device=dev),             # the head's output, rounded to fp32
+        }
+
+    def _check(self, H: int, W: int, K, bl_fx: float) -> None:
+        st = self._st
+        assert (H, W) == st["shape"], f"image shape changed since the CUDA graph was captured: {(H, W)} != {st['shape']}"
+        assert K == st["K"], "camera intrinsics changed since the CUDA graph was captured"
+        assert bl_fx == st["bl_fx"], "camera baseline * fx changed since the CUDA graph was captured"
+
+    def _upload(self, stereo) -> int:
+        """L(t), R(t) -> dimg on the current stream; returns 1 if the host waited for a staging buffer"""
+        st, dimg = self._st, self._st["dimg"]
+        imgs = (stereo.imageL, stereo.imageR)
+        if all(t.is_cuda or t.is_pinned() for t in imgs):
+            for i, t in enumerate(imgs):
+                dimg[i:i + 1].copy_(t, non_blocking=True)
+            return 0
+        if self._staging is None:
+            self._staging = [torch.empty(dimg.shape, dtype=torch.float32).pin_memory() for _ in range(2)]
+        slot = self.num_keyframes & 1
+        waited = 0
+        ev = self._staged[slot]
+        if ev is not None and not ev.query():       # the upload two keyframes ago still reads this buffer
+            ev.synchronize()
+            waited = 1
+        buf = self._staging[slot]
+        for i, t in enumerate(imgs):
+            buf[i:i + 1].copy_(t)
+        dimg.copy_(buf, non_blocking=True)
+        ev = self._staged[slot] = torch.cuda.Event()
+        ev.record()
+        return waited
+
+    def _networks(self) -> torch.Tensor:
+        """both branches, joined, and the pose network up to fc1 (returned); on the current stream"""
+        st, ops = self._st, self.ops
+        main = torch.cuda.current_stream()
+        self.side.wait_stream(main)
+        with _deterministic_cudnn():
+            with torch.cuda.stream(self.side):
+                self.matcher._run(st["mimg"], st["flow"], st["mmargin"], st["mcrop"])
+            self.depth._run(st["dst"])
+        main.wait_stream(self.side)
+        ops.posenet_input(st["flow"], st["dst"]["depth"], st["bl_fx"], st["inp"])
+        return self.motion.net.body(st["inp"])
+
+    def _keyframe(self) -> None:
+        """one keyframe's work after the upload: L(t-1), L(t) into the matcher's input, the networks, the head"""
+        st = self._st
+        st["mimg"][0].copy_(st["mimg"][1])
+        st["mimg"][1].copy_(st["dimg"][0])
+        fc1 = self._networks()
+        self.motion.head(fc1, st["prev"], st["next"])
+        st["pose"].copy_(st["next"])
+        st["prev"].copy_(st["pose"])
+
+    def _capture(self):
+        """warm up the networks (cuDNN's algorithm choice) outside the capture, then capture `_keyframe`; returns a
+        callable that replays it"""
+        ops = self.ops
+        warm = torch.cuda.Stream(self.device)
+        warm.wait_stream(torch.cuda.current_stream())
+        with torch.cuda.stream(warm):
+            self._networks()
+        torch.cuda.current_stream().wait_stream(warm)
+        graph = torch.cuda.CUDAGraph()
+        n0 = ops.LAUNCHES[0]
+        with torch.cuda.graph(graph):
+            self._keyframe()
+        launches = ops.LAUNCHES[0] - n0
+
+        def replay():
+            graph.replay()
+            ops.LAUNCHES[0] += launches
+        return replay
+
+    @torch.inference_mode()
+    def run(self, frame) -> None:
+        stereo = frame.stereo
+        record = {"K": stereo.K, "baseline": stereo.baseline, "time_ns": stereo.time_ns}
+        if frame.frame_idx % self.keyframe_freq != 0:
+            assert self.frames, "the first frame must be a keyframe"
+            prev = self.frames[-1]
+            self.frames.append(dict(record, T_BS=prev["T_BS"], need_interp=True, row=prev["row"]))
+            self.host_waits.append(0)
+            return
+        H, W = stereo.imageL.shape[-2:]
+        assert stereo.imageL.size(0) == 1 and stereo.imageR.size(0) == 1, \
+            "The interface will not handle batch dimension correctly."
+        assert tuple(stereo.imageR.shape[-2:]) == (H, W), "both images must have the same size"
+        first = self._st is None
+        if first:
+            self._setup(stereo, H, W)
+        else:
+            _, K, bl_fx = self.motion._camera(stereo)
+            self._check(H, W, K, bl_fx)
+        st, k = self._st, self.num_keyframes
+        if k == self.traj.size(0):
+            grown = torch.empty((2 * k, 7), dtype=torch.float32, device=self.device)
+            grown[:k].copy_(self.traj)
+            self.traj = grown
+        waited = self._upload(stereo)
+        if first:
+            st["mimg"][1].copy_(st["dimg"][0])
+            st["pose"].zero_()[6].fill_(1.0)                  # the identity, [t, q_xyzw]
+            st["prev"].copy_(st["pose"])
+        else:
+            kernel = bool(torch.backends.cudnn.allow_tf32)        # B200_TartanVODepth's head path for this flag
+            if kernel != st["dst"]["kernel"]:
+                st["dst"]["kernel"], self._graph = kernel, None
+            if not self.cuda_graph:
+                self._keyframe()
+            else:
+                if self._graph is None:
+                    self._graph = self._capture()
+                self._graph()
+        self.traj[k].copy_(st["pose"])
+        self.frames.append(dict(record, T_BS=stereo.T_BS, need_interp=False, row=k))
+        self.num_keyframes = k + 1
+        self.host_waits.append(waited)
+
+    def finish(self) -> tuple[torch.Tensor, torch.Tensor]:
+        """(F, 7) fp32 poses [t, q_xyzw] and (F,) bool need_interp, on the host; waits for the device once"""
+        torch.cuda.current_stream().synchronize()
+        traj = self.traj[:self.num_keyframes].cpu()
+        rows = torch.tensor([f["row"] for f in self.frames], dtype=torch.long)
+        interp = torch.tensor([f["need_interp"] for f in self.frames], dtype=torch.bool)
+        return traj[rows], interp

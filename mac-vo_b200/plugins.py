@@ -20,6 +20,7 @@
     B200_TartanMotionNet             IMotionModel       replaces TartanMotionNet (MotionModel.py:89-116)
     B200_TartanVOMatcher             IMatcher           replaces TartanVOMatcher (Frontend/Matching.py:199-230)
     B200_TartanVODepth               IStereoDepth       replaces TartanVODepth (Frontend/StereoDepth.py:186-229)
+    B200_TartanVO                    IOdometry          replaces TartanVO (Odometry/BaselineTartanVO.py:12-80)
 
 Same constructor signature (`__init__(config: SimpleNamespace)`), same `is_valid_config` contract
 (unknown keys are an error), same argument meaning and return types as the classes they replace; class
@@ -1287,6 +1288,105 @@ class B200_TartanVODepth(IStereoDepth):
         cls._enforce_config_spec(config, spec)
 
 
+# ================================================================================================
+# TartanVO baseline driver
+# ================================================================================================
+_IOdometry = object
+if _REF:
+    try:    # receive_frames (poses.npy, tensor_map.npz) comes from MAC-VO's own IOdometry
+        from Odometry.Interface import IOdometry as _IOdometry  # type: ignore
+        from Module.Map import VisualMap as _VisualMap, FrameNode as _FrameNode  # type: ignore
+    except ImportError:
+        _IOdometry = object
+
+
+class B200_TartanVO(_IOdometry):
+    """Drop-in for the TartanVO baseline's driver (Odometry/BaselineTartanVO.TartanVO): the same Odometry section, the same
+    per-frame poses and map, with every network on the device through `pipeline.FusedTartanVO` (see there for what runs
+    where). This class only builds the driver from the config and writes its trajectory in MAC-VO's map format.
+
+    It differs from the reference driver in what it does not do: it names no "Naive" map processor (the reference's, which
+    MAC-VO does not define; `terminate()` leaves the trajectory as a no-op processor would), its first pose has the map's
+    leading dimension, it runs neither the depth network's covariance decoder (whatever `depth.args.cov_mode` says) nor
+    the first frame's depth, and all frames must keep one image shape and camera."""
+
+    MATCH, DEPTH = "B200_TartanVOMatcher", "B200_TartanVODepth"
+
+    def __init__(self, match_estimator: "B200_TartanVOMatcher", depth_estimator: "B200_TartanVODepth",
+                 keyframe_freq: int, motion: "B200_TartanMotionNet", cuda_graph: bool = True):
+        if _IOdometry is not object:
+            super().__init__()
+        from .pipeline import FusedTartanVO
+        self.fused = FusedTartanVO(match_estimator, depth_estimator, motion, keyframe_freq, cuda_graph)
+        self._map = None
+
+    @classmethod
+    def from_config(cls, cfg: SimpleNamespace, seq=None) -> "B200_TartanVO":
+        """`cfg` is the Odometry section (or a whole experiment config holding one); `seq` is not read"""
+        cfg = getattr(cfg, "Odometry", cfg)
+        cls.is_valid_config(cfg)
+        depth_args = SimpleNamespace(**dict(vars(cfg.depth.args), cov_mode="None"))
+        freq = cfg.keyframe.args.keyframe_freq if cfg.keyframe.type == "UniformKeyframe" else 1
+        graph = bool(getattr(cfg.match.args, "cuda_graph", True)) and bool(getattr(cfg.depth.args, "cuda_graph", True))
+        return cls(B200_TartanVOMatcher(cfg.match.args), B200_TartanVODepth(depth_args), freq,
+                   B200_TartanMotionNet(cfg.tartanvo), cuda_graph=graph)
+
+    @torch.inference_mode()
+    def run(self, frame) -> None:
+        self._map = None
+        self.fused.run(frame)
+
+    def get_map(self):
+        """MAC-VO's VisualMap (a namespace with the same `frames.data` columns without MAC-VO), built once from the device
+        trajectory: per frame K, baseline, need_interp, time_ns, pose (fp32 [t, q_xyzw]) and T_BS"""
+        if self._map is None:
+            poses, interp = self.fused.finish()
+            fr = self.fused.frames
+            as7 = lambda t: (t.tensor() if hasattr(t, "ltype") else torch.as_tensor(t)).reshape(-1, 7).float().cpu()
+            data = {
+                "K": torch.cat([f["K"].reshape(-1, 3, 3).float().cpu() for f in fr]),
+                "baseline": torch.cat([torch.as_tensor(f["baseline"]).reshape(-1).float().cpu() for f in fr]),
+                "need_interp": interp,
+                "time_ns": torch.cat([torch.as_tensor(f["time_ns"], dtype=torch.long).reshape(-1) for f in fr]),
+                "pose": poses,
+                "T_BS": torch.cat([as7(f["T_BS"]) for f in fr]),
+            }
+            if _IOdometry is not object:
+                self._map = _VisualMap()
+                self._map.frames.push(_FrameNode.init(data))
+            else:
+                self._map = SimpleNamespace(frames=SimpleNamespace(
+                    data={k: SimpleNamespace(tensor=v) for k, v in data.items()}))
+        return self._map
+
+    def terminate(self) -> None:
+        if _IOdometry is not object:
+            super().terminate()
+
+    @classmethod
+    def is_valid_config(cls, config: SimpleNamespace | None) -> None:
+        assert config is not None
+        for key, want, plugin in (("match", cls.MATCH, B200_TartanVOMatcher), ("depth", cls.DEPTH, B200_TartanVODepth)):
+            sec = getattr(config, key, None)
+            if sec is None or getattr(sec, "type", None) != want:
+                raise ValueError(f"B200_TartanVO: Odometry.{key}.type must be {want}, got "
+                                 f"{getattr(sec, 'type', None)!r}")
+            plugin.is_valid_config(sec.args)
+        B200_TartanMotionNet.is_valid_config(config.tartanvo)
+        kf = config.keyframe
+        if kf.type == "UniformKeyframe":
+            _local._Registry._enforce_config_spec(kf.args, {"keyframe_freq": lambda f: isinstance(f, int) and f >= 1})
+        elif kf.type == "AllKeyframe":
+            _local._Registry._enforce_config_spec(kf.args, {})
+        else:
+            raise ValueError(f"B200_TartanVO: Odometry.keyframe.type must be UniformKeyframe or AllKeyframe, got "
+                             f"{kf.type!r}")
+        spec = {k: (lambda v: True) for k in ("match", "depth", "tartanvo", "keyframe")}
+        if "name" in vars(config):
+            spec["name"] = lambda n: isinstance(n, str)
+        _local._Registry._enforce_config_spec(config, spec)
+
+
 PLUGINS = {
     "frontend": B200_FlowFormerCovFrontend,
     "frontend_plain": B200_FlowFormerFrontend,
@@ -1304,4 +1404,5 @@ PLUGINS = {
     "motion": B200_TartanMotionNet,
     "matcher_tartanvo": B200_TartanVOMatcher,
     "depth_tartanvo": B200_TartanVODepth,
+    "odometry_tartanvo": B200_TartanVO,
 }
