@@ -183,6 +183,18 @@ int macvo_match_covariance(const void* kp, int kp_is_int64, int k, const float* 
                            float fx, float fy, float cx, float cy, int kernel_size, float min_flow_cov,
                            float min_depth_cov, float match_cov_default, double* out_cov, float* out_point,
                            int* status, void* stream);
+/* GaussianMixtureCovariance.estimate (Project2to3.py:194-272, gaussian_mixture_mean_var Utility/Math.py:66-93): the
+ * arguments of macvo_match_covariance, plus depth_cov (h,w) fp32, the stereo network's per-pixel depth variance
+ * (depth_est.cov, required: the reference asserts it). The same Gaussian weights p over the patch; p < 1e-3 becomes 0
+ * (NaN stays NaN) and the rest is renormalised; mean = sum p d (the depth of the projection), variance =
+ * (sum p (depth_cov + d^2) - mean^2) / 2, replaced by depth_var when flow_cov is NULL and depth_var is given. The
+ * variance is NOT clamped (the reference never reads min_depth_cov, so there is no such argument): fp32 cancellation
+ * can leave it slightly negative. A NaN depth or variance tap anywhere in the patch makes the matrix NaN. */
+int macvo_gaussian_mixture_covariance(const void* kp, int kp_is_int64, int k, const float* depth, const float* depth_cov,
+                                      int h, int w, float* flow_cov, long long flow_cov_row_stride,
+                                      long long flow_cov_col_stride, const float* depth_var, float fx, float fy, float cx,
+                                      float cy, int kernel_size, float min_flow_cov, float match_cov_default,
+                                      double* out_cov, float* out_point, int* status, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * (a14)+(a15) two-frame pose-graph optimisation — replaces TwoFrame_PGO._optimize
@@ -435,15 +447,19 @@ int macvo_cov_sanity_filter(const double* obs1_cov, const double* obs2_cov, int 
  *   [37c+4,46c+4) cov_Tw (c,3,3)        -> `packed` must hold macvo_observe_packed_doubles(capacity, 1) = 46c + 4 doubles.
  * macvo_observe_packed_doubles(capacity, 0) = 31c + 4.
  *
- * The covariance model of the ablation configs (Module/Covariance/Project2to3.py:48-57, 281-323); all zero = MatchCovariance
- * without modifiers, exactly the behaviour above:
- *   cov_model     MACVO_COV_MATCH, or MACVO_COV_IDENTITY (NoCovariance: no depth taps, the uv-covariance columns hold the
- *                 network's values unclamped, status bit 0 is never set, both 3x3 covariances are the identity);
+ * The covariance model (Module/Covariance/Project2to3.py:48-57, 194-272, 281-323); all zero = MatchCovariance without
+ * modifiers, exactly the behaviour above:
+ *   cov_model     MACVO_COV_MATCH, MACVO_COV_IDENTITY (NoCovariance: no depth taps, the uv-covariance columns hold the
+ *                 network's values unclamped, status bit 0 is never set, both 3x3 covariances are the identity), or
+ *                 MACVO_COV_GAUSSIAN_MIXTURE (GaussianMixtureCovariance, see macvo_gaussian_mixture_covariance: depth_cov0
+ *                 / depth_cov1 are the variance maps of frame 0 / 1 and must both be given, else MACVO_E_ARG; its
+ *                 covariances can be NaN, which the sanity filter drops);
  *   cov_ops[0..n_cov_ops)  modifiers in the order they apply (innermost wrapper first), in float64 on the widened fp32
  *                 covariances, BEFORE the sanity filter, the obs1_covTc / obs2_covTc columns and cov_Tw (see macvo_cov_modify).
  * Setting only these fields (no filter, icp 0) keeps the 31c + 4 layout and applies the sanity filter alone. */
 #define MACVO_COV_MATCH 0
 #define MACVO_COV_IDENTITY 1
+#define MACVO_COV_GAUSSIAN_MIXTURE 2
 #define MACVO_COV_DIAGONALIZE 1
 #define MACVO_COV_NORMALIZE 2
 #define MACVO_COV_MAX_OPS 2
@@ -480,7 +496,9 @@ int macvo_observe_pack(const int64_t* kp0_uv, int k, int capacity, const float* 
  *     icp columns pixel1_d_cov / pixel2_d_cov when ext->depth_cov0 / depth_cov1 are NULL, as above.
  *   - MACVO_COV_MATCH: MatchCovariance.estimate with flow_cov None for kp1 (Project2to3.py:128-135): its 2x2 flow
  *     covariance is match_cov_default * [1, 1, 0] WITHOUT the min_flow_cov^2 clamp; kp0 keeps the clamped default.
- *   - MACVO_COV_IDENTITY: unchanged (identity covariances). */
+ *   - MACVO_COV_IDENTITY: unchanged (identity covariances).
+ *   - MACVO_COV_GAUSSIAN_MIXTURE: kp1's flow covariance as for MACVO_COV_MATCH, and its variance is depth_cov1 at kp1
+ *     (Project2to3.py:254-255: no flow_cov, a depth_cov given). */
 
 /* ------------------------------------------------------------------------------------------------
  * (f2) decoder token path of one refinement iteration as one kernel — replaces flow_token_encoder (decoder.py:112-116),

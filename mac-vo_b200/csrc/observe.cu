@@ -13,8 +13,9 @@
 //                    all inside ONE buffer so that a single asynchronous device->host copy ships a frame's
 //                    observations; the survivor count stays on the device (pgo_lm_kernel reads it there).
 //
-// With a macvo_observe_ext_t the covariance model of the ablation configs replaces MatchCovariance: NoCovariance (identity,
-// no depth taps) and the Diagonalize / Normalize modifiers (cov_modify9, shared with macvo_cov_modify).
+// With a macvo_observe_ext_t another covariance model replaces MatchCovariance: NoCovariance (identity, no depth taps),
+// GaussianMixtureCovariance (mixture_cov_warp on the depth and depth-covariance maps) and the Diagonalize / Normalize
+// modifiers (cov_modify9, shared with macvo_cov_modify).
 //
 // Arithmetic: fp32 in the reference's operation order (explicit round-to-nearest intrinsics, no contraction), widened
 // to fp64 exactly where the reference calls `.double()`.
@@ -43,6 +44,7 @@ struct ObserveArgs {
     const float* depth_cov1;
     float* rex;                    // (k, REX) extension records
     int identity;                  // NoCovariance: no depth taps, raw uv covariances, identity 3x3 covariances
+    int mixture;                   // GaussianMixtureCovariance: depth_cov0 / depth_cov1 are the variance patches
     int n_ops, op0, op1;           // covariance modifiers, op0 first
     double* rcov;                  // (k, RCOV) modified covariances (n_ops > 0 only)
 };
@@ -173,20 +175,30 @@ observe_kernel(ObserveArgs A, float* __restrict__ rec, int* __restrict__ status)
 #pragma unroll
         for (int e = 0; e < 6; ++e) c0[e] = c1[e] = (e == 0 || e == 3 || e == 5) ? 1.f : 0.f;
     } else {
+        // the covariance estimate of one frame's keypoint: MatchCovariance, or GaussianMixtureCovariance on that frame's
+        // depth-covariance map
+        auto estimate = [&](float u, float v, long long ul, long long vl, const float* depth, const float* dvar, float su,
+                            float sv, float suv_, bool override_var, float depth_var, const macvo::CovParams& P, float* s6) {
+            return A.mixture ? macvo::mixture_cov_warp(u, v, ul, vl, depth, dvar, A.h, A.w, su, sv, suv_, override_var,
+                                                       depth_var, P, lane, s6)
+                             : macvo::match_cov_warp(u, v, ul, vl, depth, A.h, A.w, su, sv, suv_, false, 0.f, P, lane, s6);
+        };
         // frame-0 keypoints: constant quantisation covariance, clamped like any flow_cov (Project2to3.py:130-133)
         const float s0 = fmaxf(A.match_cov_default, A.min_flow_var);
-        oob = macvo::match_cov_warp((float)u0, (float)v0, u0, v0, A.depth0, A.h, A.w, s0, s0, 0.f, false, 0.f, A.P0, lane, c0);
+        oob = estimate((float)u0, (float)v0, u0, v0, A.depth0, A.depth_cov0, s0, s0, 0.f, false, 0.f, A.P0, c0);
         if (no_cov) {
-            // frame-1 keypoints without a network covariance: MatchCovariance's own default, NOT clamped
-            // (Project2to3.py:128-135); the packed column keeps the placeholder
+            // frame-1 keypoints without a network covariance: the model's own default, NOT clamped
+            // (Project2to3.py:128-135, 212-218); the packed column keeps the placeholder. The mixture then takes kp1's
+            // depth_cov as its variance (Project2to3.py:254-255)
             const float s1 = A.match_cov_default;
-            oob |= macvo::match_cov_warp(u1, v1, ul1, vl1, A.depth1, A.h, A.w, s1, s1, 0.f, false, 0.f, A.P1, lane, c1);
+            oob |= estimate(u1, v1, ul1, vl1, A.depth1, A.depth_cov1, s1, s1, 0.f, true, A.mixture ? A.depth_cov1[p1] : 0.f,
+                            A.P1, c1);
             suu = svv = -1.f;
         } else {
             // frame-1 keypoints: the network's match covariance at the source pixel, clamped in place
             suu = (a != a) ? a : fmaxf(a, A.min_flow_var);
             svv = (b != b) ? b : fmaxf(b, A.min_flow_var);
-            oob |= macvo::match_cov_warp(u1, v1, ul1, vl1, A.depth1, A.h, A.w, suu, svv, suv, false, 0.f, A.P1, lane, c1);
+            oob |= estimate(u1, v1, ul1, vl1, A.depth1, A.depth_cov1, suu, svv, suv, false, 0.f, A.P1, c1);
         }
         if (lane != 0) return;
     }
@@ -438,9 +450,12 @@ extern "C" int macvo_observe_pack(const int64_t* kp0_uv, int k, int capacity, co
         return MACVO_E_ARG;
     if (workspace_bytes < macvo_observe_workspace_bytes(capacity)) return MACVO_E_WORKSPACE;
     if (ext && ext->simple_depth && !(ext->min_depth <= ext->max_depth)) return MACVO_E_ARG;
-    if (ext && ((ext->cov_model != MACVO_COV_MATCH && ext->cov_model != MACVO_COV_IDENTITY) ||
+    if (ext && ((ext->cov_model != MACVO_COV_MATCH && ext->cov_model != MACVO_COV_IDENTITY &&
+                 ext->cov_model != MACVO_COV_GAUSSIAN_MIXTURE) ||
                 !valid_cov_ops(ext->cov_ops, ext->n_cov_ops)))
         return MACVO_E_ARG;
+    // GaussianMixtureCovariance asserts depth_est.cov is not None (Project2to3.py:206)
+    if (ext && ext->cov_model == MACVO_COV_GAUSSIAN_MIXTURE && (!ext->depth_cov0 || !ext->depth_cov1)) return MACVO_E_ARG;
     ObserveArgs A;
     A.kp0 = kp0_uv; A.k = k; A.flow = flow; A.match_cov = match_cov; A.depth0 = depth0; A.depth1 = depth1;
     A.disparity1 = disparity1; A.disp_unc1 = disp_unc1; A.h = h; A.w = w; A.edge = edge_width;
@@ -456,6 +471,7 @@ extern "C" int macvo_observe_pack(const int64_t* kp0_uv, int k, int capacity, co
     A.depth_cov0 = ext ? ext->depth_cov0 : nullptr; A.depth_cov1 = ext ? ext->depth_cov1 : nullptr;
     A.rex = rec + (size_t)capacity * REC;
     A.identity = ext && ext->cov_model == MACVO_COV_IDENTITY;
+    A.mixture = ext && ext->cov_model == MACVO_COV_GAUSSIAN_MIXTURE;
     A.n_ops = ext ? ext->n_cov_ops : 0;
     A.op0 = A.n_ops > 0 ? ext->cov_ops[0] : 0;
     A.op1 = A.n_ops > 1 ? ext->cov_ops[1] : 0;

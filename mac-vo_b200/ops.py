@@ -70,6 +70,9 @@ EXPORTS = {
     "macvo_match_covariance": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p,
                                          C.c_longlong, C.c_longlong, C.c_void_p]
                                + [C.c_float] * 4 + [C.c_int] + [C.c_float] * 3 + [C.c_void_p] * 4),
+    "macvo_gaussian_mixture_covariance": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
+                                                    C.c_void_p, C.c_longlong, C.c_longlong, C.c_void_p]
+                                          + [C.c_float] * 4 + [C.c_int] + [C.c_float] * 2 + [C.c_void_p] * 4),
     "macvo_pgo_solve": (C.c_int, [C.c_void_p] * 5 + [C.c_int] + [C.c_void_p] * 2 + [C.POINTER(_PgoParams)]
                         + [C.c_void_p] * 2),
     "macvo_pgo_solve_graph": (C.c_int, [C.c_int] + [C.c_void_p] * 8 + [C.c_int] + [C.c_void_p] * 2 + [C.POINTER(_PgoParams)]
@@ -509,13 +512,17 @@ def retrieve_pixels(pixel_uv: Tensor, scalar_map: Tensor) -> Tensor:
 def match_covariance(kp: Tensor, depth_map: Tensor, flow_cov: Tensor | None, fx: float, fy: float, cx: float,
                      cy: float, kernel_size: int = 31, min_flow_cov: float = 0.25, min_depth_cov: float = 0.05,
                      match_cov_default: float = 0.25, want_point: bool = False, depth_cov: Tensor | None = None,
-                     out_cov: Tensor | None = None):
+                     out_cov: Tensor | None = None, depth_cov_map: Tensor | None = None):
     """-> (cov (K,3,3) float64 on the device, point (K,3) fp32 or None, status int32 tensor).
 
     flow_cov: (K,3) fp32 CUDA tensor with ANY strides (MAC-VO passes the transposed view of a (3,K) gather,
     Odometry/MACVO.py:231-232); its first two columns are clamped in place in the caller's storage like the reference.
     depth_cov: (K,) per-keypoint depth variance, only used when flow_cov is None (Project2to3.py:163-171).
-    out_cov: optional preallocated (K,3,3) float64 CUDA view to fill (e.g. a slice of a packed buffer)."""
+    out_cov: optional preallocated (K,3,3) float64 CUDA view to fill (e.g. a slice of a packed buffer).
+    depth_cov_map: the (1,1,H,W) per-pixel depth variance of the stereo network (`depth_est.cov`). Given, the model is
+    GaussianMixtureCovariance (Project2to3.py:194-272, macvo_gaussian_mixture_covariance) instead of MatchCovariance:
+    each tap a Gaussian with its own variance, the mixture's mean and halved variance, which is not clamped (the
+    reference never reads min_depth_cov)."""
     dm = _arg(depth_map, F32, "match_covariance depth", copy=True)
     if kp.dtype not in (torch.int64, torch.float32):
         kp = kp.float()
@@ -531,14 +538,19 @@ def match_covariance(kp: Tensor, depth_map: Tensor, flow_cov: Tensor | None, fx:
     dv = None
     if fc is None and depth_cov is not None:
         dv = _arg(depth_cov.reshape(-1), F32, "match_covariance depth_cov (one value per keypoint)", numel=K, copy=True)
+    vm = _arg(depth_cov_map, F32, "match_covariance depth_cov_map", numel=H * W, copy=True, optional=True)
     if out_cov is None:
         cov = torch.empty((K, 3, 3), dtype=torch.float64, device=dm.device)
     else:
         cov = _arg(out_cov, F64, "match_covariance out_cov", shape=(K, 3, 3))
     pt = torch.empty((K, 3), dtype=torch.float32, device=dm.device) if want_point else None
     status = torch.zeros((1,), dtype=torch.int32, device=dm.device)
-    _launch("macvo_match_covariance", kpd, int(kpd.dtype == torch.int64), K, dm, H, W, fc, rs, cs, dv, fx, fy, cx, cy,
-            kernel_size, min_flow_cov, min_depth_cov, match_cov_default, cov, pt, status)
+    if vm is None:
+        _launch("macvo_match_covariance", kpd, int(kpd.dtype == torch.int64), K, dm, H, W, fc, rs, cs, dv, fx, fy, cx, cy,
+                kernel_size, min_flow_cov, min_depth_cov, match_cov_default, cov, pt, status)
+    else:
+        _launch("macvo_gaussian_mixture_covariance", kpd, int(kpd.dtype == torch.int64), K, dm, vm, H, W, fc, rs, cs, dv, fx,
+                fy, cx, cy, kernel_size, min_flow_cov, match_cov_default, cov, pt, status)
     return cov, pt, status
 
 
@@ -673,7 +685,8 @@ def cov_sanity_filter(obs1_cov: Tensor, obs2_cov: Tensor) -> Tensor:
     return good.bool()
 
 
-COV_MODELS = {"match": 0, "identity": 1}              # macvo_observe_ext_t.cov_model (MACVO_COV_MATCH / _IDENTITY)
+COV_MODELS = {"match": 0, "identity": 1, "mixture": 2}   # macvo_observe_ext_t.cov_model (MACVO_COV_MATCH / _IDENTITY /
+                                                         # _GAUSSIAN_MIXTURE)
 COV_OPS = {"diagonalize": 1, "normalize": 2}          # MACVO_COV_DIAGONALIZE / MACVO_COV_NORMALIZE
 
 
@@ -702,8 +715,9 @@ def observe_pack(buf: ObservationBuffers, kp0_uv: Tensor, flow: Tensor, match_co
 
     ext (None: CovarianceSanityFilter only) = macvo_observe_ext_t as a dict: depth_cov0 / depth_cov1 ((1,1,H,W) fp32 CUDA
     or None), simple_depth (bool), min_depth / max_depth (floats, rounded to fp32 like the reference's comparisons),
-    front_of_cam (bool), icp (bool: pack the "icp" graph's columns; needs an extended buffer), cov_model ("match" or
-    "identity", the NoCovariance model) and cov_ops (modifier names of COV_OPS, innermost first).
+    front_of_cam (bool), icp (bool: pack the "icp" graph's columns; needs an extended buffer), cov_model ("match",
+    "identity", the NoCovariance model, or "mixture", GaussianMixtureCovariance on depth_cov0 / depth_cov1, which it then
+    requires) and cov_ops (modifier names of COV_OPS, innermost first).
 
     match_cov and disp_unc1 both None: a frontend without covariance maps (pixel2_uv_cov / pixel2_disp_cov hold -1, kp1's
     MatchCovariance uses match_cov_default unclamped; include/macvo_b200.h)."""
@@ -740,6 +754,8 @@ def observe_pack(buf: ObservationBuffers, kp0_uv: Tensor, flow: Tensor, match_co
         model = ext.get("cov_model", "match")
         if model not in COV_MODELS:
             raise MacvoB200Error(f"observe_pack: cov_model must be one of {sorted(COV_MODELS)}, got {model!r}")
+        if model == "mixture" and (dc[0] is None or dc[1] is None):
+            raise MacvoB200Error("observe_pack: cov_model 'mixture' needs the depth-covariance maps depth_cov0 and depth_cov1")
         ops_ = tuple(ext.get("cov_ops", ()))
         xs.cov_model, xs.cov_ops, xs.n_cov_ops = COV_MODELS[model], _cov_ops(ops_, "observe_pack"), len(ops_)
     buf.status.zero_()

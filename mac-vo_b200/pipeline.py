@@ -229,9 +229,10 @@ class FusedTwoFrameOdometry:
 
     The ablation back ends: `kp_selector` may be a B200_RandomSelector, whose keypoints are drawn on the device with no
     candidate count, so that with mapping off a frame has NO host synchronisation (`host_waits` records each frame's
-    count). `cov_model` may be B200_NoCovariance or B200_Modifier_Diagonalize / _Normalize around a B200 model
-    (`plugins.cov_spec`): observe_pack applies the model, and the mapping branch gets the same covariances. With
-    B200_NoCovariance the chain may leave out B200_CovarianceSanityFilter (`plugins.check_sanity_chain`).
+    count). `cov_model` may be B200_NoCovariance, B200_GaussianMixtureCovariance or B200_Modifier_Diagonalize / _Normalize
+    around a B200 model (`plugins.cov_spec`): observe_pack applies the model, and the mapping branch gets the same
+    covariances. With B200_NoCovariance the chain may leave out B200_CovarianceSanityFilter (`plugins.check_sanity_chain`).
+    B200_GaussianMixtureCovariance reads the frontend's depth covariance maps: a frontend without them is refused here.
 
     A frontend without covariance maps (B200_FlowFormerFrontend, the Vanilla ablation) hands observe_pack NULL maps: the
     packed pixel2_uv_cov / pixel2_disp_cov columns hold MatchObs' -1 placeholder."""
@@ -257,8 +258,12 @@ class FusedTwoFrameOdometry:
         self.mapping, self.min_num_point, self.num_map_point = mapping and map_selector is not None, min_num_point, num_map_point
         self.keep_debug = keep_debug
         from .plugins import B200_RandomSelector, check_sanity_chain, cov_spec
-        _, self.cov_ops, params = cov_spec(cov_model)
-        self.cov_identity = params is None
+        base, self.cov_ops, params = cov_spec(cov_model)
+        self.cov_kind = base.COV_MODEL
+        self.cov_identity = self.cov_kind == "identity"
+        if self.cov_kind == "mixture" and not getattr(frontend, "provide_cov", (True, True))[0]:
+            raise ValueError(f"{type(base).__name__} needs the depth covariance (depth_est.cov), and "
+                             f"{type(frontend).__name__} provides none")
         check_sanity_chain(outlier_filter, covariance_finite=self.cov_identity)
         self.device = kp_selector.device
         self.random_kp = isinstance(kp_selector, B200_RandomSelector)   # drawn on the device: no candidate count to wait for
@@ -266,8 +271,8 @@ class FusedTwoFrameOdometry:
         # mapping branch's covariance kernel to the point gather at the centre pixel
         self.cov_args = params or dict(kernel_size=1, min_flow_cov=0.25, min_depth_cov=0.05)
         self.cov_ext = {}
-        if self.cov_identity or self.cov_ops:
-            self.cov_ext = {"cov_model": "identity" if self.cov_identity else "match", "cov_ops": list(self.cov_ops)}
+        if self.cov_kind != "match" or self.cov_ops:
+            self.cov_ext = {"cov_model": self.cov_kind, "cov_ops": list(self.cov_ops)}
         self.cluster = int(getattr(optimizer, "context", {}).get("cluster", 0)) if hasattr(optimizer, "context") else 0
         icp = self.graph_type == "icp"
         self.obs = [ops.ObservationBuffers(num_point, self.device, extended=icp) for _ in range(2)]      # double buffered
@@ -398,10 +403,12 @@ class FusedTwoFrameOdometry:
             if n_map:   # constant quantisation covariance for manually selected pixels, clamped like any flow_cov
                 sig = max(float(torch.tensor(self.match_cov_default, dtype=torch.float32)),
                           float(torch.tensor(self.cov_args["min_flow_cov"], dtype=torch.float32) ** 2))
+                # GaussianMixtureCovariance mixes over depth0.cov (MACVO.py:316-324)
                 _, pt, _ = ops.match_covariance(map0_uv, depth0.depth, None, *i0, kernel_size=self.cov_args["kernel_size"],
                                                 min_flow_cov=self.cov_args["min_flow_cov"],
                                                 min_depth_cov=self.cov_args["min_depth_cov"], match_cov_default=sig,
-                                                want_point=True, out_cov=self.map_cov[slot][:n_map])
+                                                want_point=True, out_cov=self.map_cov[slot][:n_map],
+                                                depth_cov_map=depth0.cov if self.cov_kind == "mixture" else None)
                 if self.cov_identity:   # NoCovariance: the covariances are the identity, the points as above
                     self.map_cov[slot][:n_map].copy_(self._eye.expand(n_map, 3, 3))
                 if self.cov_ops:

@@ -9,6 +9,7 @@
     B200_RandomSelector              IKeypointSelector  replaces RandomSelector (KeypointSelector.py:103-118)
     B200_MatchCovariance             ICovariance2to3    replaces MatchCovariance (Covariance/Project2to3.py:114-182)
     B200_NoCovariance                ICovariance2to3    replaces NoCovariance (Covariance/Project2to3.py:48-57)
+    B200_GaussianMixtureCovariance   ICovariance2to3    replaces GaussianMixtureCovariance (Covariance/Project2to3.py:194-272)
     B200_Modifier_Diagonalize        ICovariance2to3    replaces Modifier_Diagonalize (Covariance/Project2to3.py:281-302)
     B200_Modifier_Normalize          ICovariance2to3    replaces Modifier_Normalize (Covariance/Project2to3.py:305-323)
     B200_CovarianceSanityFilter      IObservationFilter replaces CovarianceSanityFilter (OutlierFilter.py:91-100)
@@ -478,9 +479,11 @@ class B200_MatchCovariance(ICovariance2to3):
     tensor like the reference (its `create_3x3_matrix` assembles the result on the CPU, and
     Odometry/MACVO.py multiplies it with CPU rotations) — filled by ONE device->host copy instead of nine."""
 
+    COV_MODEL = "match"         # macvo_observe_ext_t.cov_model of this model (ops.COV_MODELS)
+
     def __init__(self, config: SimpleNamespace):
         super().__init__(config)
-        self.device = _require_cuda(config.device, "B200_MatchCovariance")
+        self.device = _require_cuda(getattr(config, "device", "cuda"), type(self).__name__)
         self.last_status: torch.Tensor | None = None
         self._status_host: torch.Tensor | None = None
 
@@ -496,15 +499,21 @@ class B200_MatchCovariance(ICovariance2to3):
         if fc is not None and not (fc.is_cuda and fc.device == self.device and fc.dtype == torch.float32):
             staged = fc.to(device=self.device, dtype=torch.float32).contiguous()
             fc = staged
+        dcm = self._depth_cov_map(depth_est)
         cov, pt, status = ops.match_covariance(
             kp.to(self.device), depth_est.depth, fc, frame.fx, frame.fy, frame.cx, frame.cy,
             kernel_size=self.config.kernel_size, min_flow_cov=self.config.min_flow_cov,
             min_depth_cov=self.config.min_depth_cov, match_cov_default=self.config.match_cov_default,
-            want_point=want_point, depth_cov=depth_cov.to(self.device) if (fc is None and depth_cov is not None) else None)
+            want_point=want_point, depth_cov=depth_cov.to(self.device) if (fc is None and depth_cov is not None) else None,
+            **({} if dcm is None else {"depth_cov_map": dcm}))
         if staged is not None:
             flow_cov.copy_(staged)
         self.last_status = status
         return cov, pt
+
+    def _depth_cov_map(self, depth_est):
+        """the per-pixel depth variance the model reads: none for MatchCovariance"""
+        return None
 
     @torch.inference_mode()
     def estimate(self, frame, kp, depth_est, depth_cov, flow_cov) -> torch.Tensor:
@@ -519,7 +528,7 @@ class B200_MatchCovariance(ICovariance2to3):
         self._status_host.copy_(self.last_status, non_blocking=True)      # rides in front of the blocking copy below
         out = cov.cpu()                                                     # ONE synchronising device->host copy
         if int(self._status_host[0]) != 0:
-            raise IndexError("MatchCovariance: a keypoint's depth patch leaves the image")
+            raise IndexError(f"{type(self).__name__[5:]}: a keypoint's depth patch leaves the image")
         return out
 
     @classmethod
@@ -533,10 +542,41 @@ class B200_MatchCovariance(ICovariance2to3):
         })
 
 
+class B200_GaussianMixtureCovariance(B200_MatchCovariance):
+    """Replacement of GaussianMixtureCovariance (Project2to3.py:194-272, "Depth + Match Covariance" in
+    Config/ConfigSpec.md): every tap of the kernel_size^2 patch is a Gaussian with the stereo network's own depth variance
+    (`depth_est.cov`), weighted like MatchCovariance's taps; the depth and its variance are that mixture's mean and
+    (halved, unclamped) variance (`ops.match_covariance` with the depth_cov_map). Needs a frontend with depth covariance.
+    Same return types, in-place clamp of `flow_cov` and IndexError as B200_MatchCovariance.
+
+    config: the reference's kernel_size (odd, 1..31), match_cov_default, min_flow_cov, min_depth_cov (required and, as in
+    the reference, never used), and an optional device (default "cuda"), so that the reference's YAML validates as is."""
+    COV_MODEL = "mixture"
+
+    def _depth_cov_map(self, depth_est):
+        if getattr(depth_est, "cov", None) is None:     # the reference asserts depth_est.cov is not None
+            raise ValueError("B200_GaussianMixtureCovariance needs the depth covariance depth_est.cov, which this frontend "
+                             "does not provide")
+        return depth_est.cov
+
+    @classmethod
+    def is_valid_config(cls, config: SimpleNamespace | None) -> None:
+        spec = {
+            "kernel_size": lambda k: isinstance(k, int) and k % 2 == 1 and 1 <= k <= 31,
+            "match_cov_default": lambda c: isinstance(c, (int, float)) and c > 0,
+            "min_depth_cov": lambda c: isinstance(c, (int, float)) and c > 0,
+            "min_flow_cov": lambda c: isinstance(c, (int, float)) and c > 0,
+        }
+        if config is not None and "device" in vars(config):
+            spec["device"] = lambda dev: isinstance(dev, str) and "cuda" in dev
+        cls._enforce_config_spec(config, spec)
+
+
 class B200_NoCovariance(ICovariance2to3):
     """Replacement of NoCovariance (Project2to3.py:48-57), the covariance model of the CovKP ablation: identity
     covariances. Like the reference it reads no depth patch and leaves `flow_cov` alone, so the MatchObs column
     `pixel2_uv_cov` keeps the network's unclamped values. config: none."""
+    COV_MODEL = "identity"
 
     def estimate(self, frame, kp, depth_est, depth_cov, flow_cov) -> torch.Tensor:
         return torch.eye(3).unsqueeze(0).repeat(kp.size(0), 1, 1).double()       # CPU float64, as the reference
@@ -606,12 +646,13 @@ def _require_b200_cov(name, who: str) -> None:
         cls = None
     if not (isinstance(cls, type) and issubclass(cls, (B200_MatchCovariance, B200_NoCovariance, _B200_CovModifier))):
         raise ValueError(f"{who}: the nested covariance model must be a B200 model (B200_MatchCovariance, "
-                         f"B200_NoCovariance or another B200 modifier), got {name!r}")
+                         f"B200_GaussianMixtureCovariance, B200_NoCovariance or another B200 modifier), got {name!r}")
 
 
 def cov_spec(cov_model) -> tuple[ICovariance2to3, list[str], dict | None]:
     """(base model, modifiers innermost first, the base model's kernel parameters or None for B200_NoCovariance) of a
-    B200 covariance model: what `macvo_observe_pack` and the fused driver's mapping branch need."""
+    B200 covariance model: what `macvo_observe_pack` and the fused driver's mapping branch need. The base model's
+    COV_MODEL names it ("match", "mixture" or "identity")."""
     ops_: list[str] = []
     m = cov_model
     while isinstance(m, _B200_CovModifier):
@@ -1395,6 +1436,7 @@ PLUGINS = {
     "mappoint": B200_MappingPointSelector,
     "cov": B200_MatchCovariance,
     "cov_none": B200_NoCovariance,
+    "cov_mixture": B200_GaussianMixtureCovariance,
     "cov_diagonalize": B200_Modifier_Diagonalize,
     "cov_normalize": B200_Modifier_Normalize,
     "keypoint_random": B200_RandomSelector,
