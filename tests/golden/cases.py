@@ -84,7 +84,9 @@ def net_inputs(B: int, H: int, W: int, seed: int = 1000) -> tuple[Tensor, Tensor
 
 
 # ---- dense post-processing -------------------------------------------------------------------------
-DENSE_CASES = {"small": (64, 96)}
+# "ragged": not a multiple of the 32x8 tile in x or y, nor of the 1024-pixel chunk (75*102 % 1024 = 482). The per-pixel
+# arithmetic does not depend on the frame size, so a small ragged shape stands in for the dataset frames here.
+DENSE_CASES = {"small": (64, 96), "ragged": (75, 102)}
 
 
 def dense_inputs(H: int, W: int, seed: int = 4) -> tuple[Tensor, Tensor]:
@@ -106,7 +108,69 @@ SELECTOR_CASES = {
     "nan": (160, 224, 128, "nan"),
     "masked": (160, 224, 128, "masked"),
     "flat": (96, 128, 50, "flat"),
+    # the shipped dataset frame sizes (EuRoC 752x480, KITTI 1241x376 and 1226x370) and a small shape ragged on all three
+    # counts: W % 32, H % 8 and H*W % 1024 are all non-zero except where noted (EuRoC: H % 8 = 0, KITTI: H % 8 = 0)
+    "euroc": (480, 752, 512, "plain"),
+    "kitti": (376, 1241, 512, "plain"),
+    "kitti00": (370, 1226, 512, "plain"),
+    "kitti00_nan": (370, 1226, 128, "nan"),
+    "ragged": (75, 102, 64, "plain"),
+    "ragged_ties": (75, 102, 4096, "ties"),
 }
+# `mask_width` of the selectors (border excluded from selection); 32 unless listed. At the dataset sizes the last partial
+# 1024-pixel chunk lies inside the last image row, which no mask width >= 1 lets through; the small ragged cases use 2
+# so that selectable candidates fall into their last partial chunk (rows 70-74 of 75).
+_SELECTOR_MASK_WIDTH = {"ragged": 2, "ragged_ties": 2, "depth_ragged": 2, "depth_ragged_ties": 2}
+
+
+def selector_mask_width(name: str) -> int:
+    return _SELECTOR_MASK_WIDTH.get(name, 32)
+
+
+def _is_ragged(H: int, W: int) -> bool:
+    return W % 32 != 0 or H % 8 != 0 or (H * W) % 1024 != 0
+
+
+def selector_plantings(H: int, W: int) -> dict:
+    """Pixels `selector_inputs` plants into a shape that does not fill the 32x8 scoring tiles / 1024-pixel compaction
+    chunks (flat row-major indices, (y, x) = divmod(p, W)):
+      edge_min    (H-1, W-1): the strict minimum of its 7x7 NMS window, which crosses the right and bottom edges;
+      nan         (H-1, W-9): a NaN flow covariance in the last partial chunk, outside edge_min's window;
+      candidates  pixels of row H-3 in the last partial chunk: strict window minima, below every unplanted quality and
+                  with depth 2.5 / depth covariance 7.6e-4 (selectable by all three selectors for mask_width <= 2).
+                  Empty where the last partial chunk does not reach row H-3 (the dataset sizes)."""
+    chunk0 = (H * W) // 1024 * 1024
+    cands = [(H - 3) * W + x for x in (8, W // 2, W - 20) if (H - 3) * W + x >= chunk0]
+    return {"edge_min": H * W - 1, "nan": H * W - 9, "candidates": cands, "last_chunk": chunk0}
+
+
+def _plant_ragged_edges(flow: Tensor, cov: Tensor, H: int, W: int) -> None:
+    pl = selector_plantings(H, W)
+    low = 2.0 ** -6                              # flow quality uu + vv = 2^-5 < 0.25, the least unplanted value
+    for p in [pl["edge_min"]] + pl["candidates"]:
+        y, x = divmod(p, W)
+        cov[1, 0, y, x] = cov[1, 1, y, x] = low
+        flow[0, 0, y, x] = -32.0                 # disparity 32 (> the 1..31 of the rest): depth 2.5, depth cov 6400/8 / 32^4
+        cov[0, 0, y, x] = 0.125
+    cov[1, 0].view(-1)[pl["nan"]] = float("nan")
+    # the plantings hold on the inputs themselves, not by assumption
+    q = cov[1, 0] + cov[1, 1]                    # flow quality uu + vv - 2 * 0 (the padded uv channel)
+    dcov = cov[0, 0] / flow[0, 0] ** 4           # depth covariance / (baseline * fx)^2
+    unplanted = torch.ones(H * W, dtype=torch.bool)
+    unplanted[[pl["edge_min"]] + pl["candidates"]] = False
+    assert pl["last_chunk"] < pl["nan"] < H * W and q.view(-1)[pl["nan"]].isnan()
+    for p in [pl["edge_min"]] + pl["candidates"]:
+        y, x = divmod(p, W)
+        win = q[max(y - 3, 0):y + 4, max(x - 3, 0):x + 4]
+        assert not win.isnan().any() and int((win <= q[y, x]).sum()) == 1, (y, x)
+        assert q[y, x] < q.view(-1)[unplanted].nan_to_num(float("inf")).min()
+        assert dcov[y, x] < dcov.view(-1)[unplanted].min()           # also the least depth covariance (depth-aware)
+        assert p >= pl["last_chunk"]
+    y, x = divmod(pl["edge_min"], W)
+    assert y + 3 >= H and x + 3 >= W                                    # window crosses the bottom and right edges
+    for p in pl["candidates"]:
+        y, x = divmod(p, W)
+        assert 2 <= x < W - 2 and 2 <= y < H - 2                        # inside a mask_width-2 border
 
 
 def selector_inputs(H: int, W: int, variant: str, seed: int = 4) -> tuple[Tensor, Tensor]:
@@ -122,11 +186,16 @@ def selector_inputs(H: int, W: int, variant: str, seed: int = 4) -> tuple[Tensor
         cov[1, 1].view(-1)[idx[:50] + 1] = float("inf")
     elif variant == "flat":    # constant quality: every pixel is its window minimum
         cov = torch.full_like(cov, 0.75)
+    if _is_ragged(H, W):
+        _plant_ragged_edges(flow, cov, H, W)
     return flow, cov
 
 
 SELECTOR_DEPTH_CASES = {"depth_small": (160, 224, 64, "plain"), "depth_cfgA": (480, 640, 512, "plain"),
-                        "depth_masked": (160, 224, 128, "masked"), "depth_nan": (160, 224, 128, "nan")}
+                        "depth_masked": (160, 224, 128, "masked"), "depth_nan": (160, 224, 128, "nan"),
+                        "depth_euroc": (480, 752, 512, "plain"), "depth_kitti": (376, 1241, 512, "plain"),
+                        "depth_kitti00": (370, 1226, 512, "plain"), "depth_kitti00_nan": (370, 1226, 128, "nan"),
+                        "depth_ragged": (75, 102, 64, "plain"), "depth_ragged_ties": (75, 102, 4096, "ties")}
 
 
 def selector_depth_inputs(H: int, W: int, variant: str):
@@ -251,29 +320,42 @@ def _typed_fields(c: dict) -> dict:
             "pts_cov": c["pts_cov"].double().numpy()}
 
 
-# ---- 640x480 / depth-12 network parity ladder (BASELINE configs[1] shape) -------------------------------------------
-CFGA = (480, 640)
+# ---- depth-12 network parity ladder: 640x480 (BASELINE configs[1] shape) and the shipped dataset frame sizes ----------
+# (H, W) of the frame. cfgA and TartanAir share 640x480; EuRoC is 752x480 (1/8 grid 60x94); KITTI is 1241x376 (padded
+# to 1248x376, 1/8 grid 47x156) and 1226x370 for sequences 00-02 (padded to 1232x376, 1/8 grid 47x154).
+LADDER_CASES = {"cfgA": (480, 640), "euroc": (480, 752), "kitti": (376, 1241), "kitti00": (370, 1226)}
+# strided samples of each stage, the same indices on both sides of the comparison: full-resolution pixel stride (phase
+# 2; 5 and 21 are coprime with 8, so every 8x8 upsampling phase is sampled), feature (channel, row, column) strides,
+# correlation (tapped row, column) strides, cost-memory (row, channel) strides and the 1/8-grid iterate stride. Coarser at
+# the dataset sizes, so that each of their fixtures stays under 0.5 MB.
+_DATASET_SAMPLE = {"px": 21, "feat": (32, 8, 14), "corr": (10, 35), "mem": (388, 8), "iter": 6}
+_LADDER_SAMPLES = {"cfgA": {"px": 5, "feat": (8, 4, 5), "corr": (5, 7), "mem": (37, 4), "iter": 2},
+                   "euroc": _DATASET_SAMPLE, "kitti": _DATASET_SAMPLE, "kitti00": _DATASET_SAMPLE}
 
 
-def cfgA_inputs() -> tuple[Tensor, Tensor]:
+def ladder_inputs(case: str = "cfgA") -> tuple[Tensor, Tensor]:
     """the `estimate_pair` batch of the bench sequence's first step: [t2.L, t1.L] vs [t2.R, t2.L] (Frontend.py:284-285)"""
     from macvo_b200 import synthetic
-    fr = synthetic.make_sequence(2, *CFGA)
+    fr = synthetic.make_sequence(2, *LADDER_CASES[case])
     return torch.cat([fr[1].imageL, fr[0].imageL]), torch.cat([fr[1].imageR, fr[1].imageL])
 
 
-def cfgA_sample(name: str, t: Tensor) -> Tensor:
-    """fixed strided samples of the per-stage tensors (keeps the fixture < 2 MB; same indices on both sides)"""
-    if name in ("flow", "cov"):                 # (2,2,480,640) full-resolution outputs: stride 5, phase 2 (all 8x8 phases hit)
-        return t[..., 2::5, 2::5]
-    if name in ("feats", "context"):            # (B,256,60,80)
-        return t[:, ::8, ::4, ::5]
+def ladder_sample(case: str, name: str, t: Tensor) -> Tensor:
+    """fixed strided samples of the per-stage tensors (`_LADDER_SAMPLES`)"""
+    s = _LADDER_SAMPLES[case]
+    if name in ("flow", "cov"):                 # (2,2,H,W) full-resolution outputs
+        return t[..., 2::s["px"], 2::s["px"]]
+    if name in ("feats", "context"):            # (B,256,H1,W1)
+        c, r, w = s["feat"]
+        return t[:, ::c, ::r, ::w]
     if name == "corr_rows":                     # (B, N/97, N) rows already strided by the tap
-        return t[:, ::5, ::7]
+        r, w = s["corr"]
+        return t[:, ::r, ::w]
     if name == "cost_memory":                   # (B*N, 8, 128)
-        return t[::37, :, ::4]
-    if name in ("flow_iter", "cov_iter"):       # (2,2,60,80) per iteration
-        return t[..., ::2, ::2]
+        r, c = s["mem"]
+        return t[::r, :, ::c]
+    if name in ("flow_iter", "cov_iter"):       # (2,2,H1,W1) per iteration
+        return t[..., ::s["iter"], ::s["iter"]]
     raise KeyError(name)
 
 

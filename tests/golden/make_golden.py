@@ -118,9 +118,10 @@ def main() -> None:
                 "flow": m.flow, "flow_cov": m.cov})
 
     # ---- selectors (a8, a8'') ---------------------------------------------------------------
-    sel = CovAwareSelector_NoDepth(SimpleNamespace(device="cpu", kernel_size=7, mask_width=32, max_match_cov=100.0))
-    mapsel = MappingPointSelector(SimpleNamespace(max_depth=5.0, max_depth_cov=0.005, mask_width=32))
     for name, (H, W, num, variant) in cases.SELECTOR_CASES.items():
+        mw = cases.selector_mask_width(name)
+        sel = CovAwareSelector_NoDepth(SimpleNamespace(device="cpu", kernel_size=7, mask_width=mw, max_match_cov=100.0))
+        mapsel = MappingPointSelector(SimpleNamespace(max_depth=5.0, max_depth_cov=0.005, mask_width=mw))
         est_flow, est_cov = cases.selector_inputs(H, W, variant)
         frame = stereo(H, W, 320.0, 0.25)
         depth = FlowFormerCovFrontend.inference_2_depth(est_flow[0:1], est_cov[0:1], frame, False)
@@ -133,9 +134,9 @@ def main() -> None:
         save(f"selector_{name}.pt", {"shape": (H, W), "num": num, "variant": variant, "kp": kp, "map_kp": mp,
                                      "input_sha": cases.sha(est_flow, est_cov)})
 
-    dsel = CovAwareSelector(SimpleNamespace(device="cpu", kernel_size=7, mask_width=32, max_depth="auto",
-                                            max_depth_cov=250.0, max_match_cov=100.0))
     for name, (H, W, num, variant) in cases.SELECTOR_DEPTH_CASES.items():
+        dsel = CovAwareSelector(SimpleNamespace(device="cpu", kernel_size=7, mask_width=cases.selector_mask_width(name),
+                                                max_depth="auto", max_depth_cov=250.0, max_match_cov=100.0))
         (f0, c0), (f1, c1) = cases.selector_depth_inputs(H, W, variant)
         frame = stereo(H, W, 320.0, 0.25)
         depth0 = FlowFormerCovFrontend.inference_2_depth(f0[0:1], c0[0:1], frame, variant == "masked")

@@ -17,11 +17,15 @@ import torch
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
 
-# the three workloads of bench.py: its CONFIGS "performant" / "fast" (build_gpu_pipeline) and SHARDED (run_sharded on one GPU)
+# the three workloads of bench.py (its CONFIGS "performant" / "fast" through build_gpu_pipeline, SHARDED through run_sharded
+# on one GPU), and the performant settings at the EuRoC (752x480) and KITTI 00-02 (1226x370) frame sizes, where the
+# 32x8 scoring tiles and 1024-pixel compaction chunks end ragged (W % 32, H % 8 and H*W % 1024 not all zero)
 WORKLOADS = {
     "performant": dict(H=480, W=640, enc_dtype="fp32", dec_dtype="fp32", num_point=200, kernel_size=7),
     "fast": dict(H=480, W=640, enc_dtype="fp16", dec_dtype="bf16", num_point=2048, kernel_size=7),
     "sharded": dict(H=720, W=1280, enc_dtype="fp32", dec_dtype="fp32", num_point=4096, kernel_size=3),
+    "euroc": dict(H=480, W=752, enc_dtype="fp32", dec_dtype="fp32", num_point=200, kernel_size=7),
+    "kitti00": dict(H=370, W=1226, enc_dtype="fp32", dec_dtype="fp32", num_point=200, kernel_size=7),
 }
 MODES = ("eager", "graph", "graph_prefetch")
 ORDER = (0, 1, 2, 1, 0, 1, 2)       # ping-pong over three frames: initialize(frames[0]), then six pairs, both directions
@@ -442,8 +446,8 @@ def test_driving_modes_agree_bit_for_bit(lib, name):
 @pytest.mark.parametrize("name", list(WORKLOADS))
 def test_selector_score_source(lib, name):
     """The frontend's dense pass scores keypoints with its 7 x 7 NMS window; the selector takes those scores through the
-    `_b200_score` token when its own kernel_size is 7 (performant, fast) and scores the map again with `score_only` when it
-    is 3 (sharded). Counted in the kernels one eager pair launched: one dense_score_kernel (the frontend's) or two."""
+    `_b200_score` token when its own kernel_size is 7 (performant, fast, euroc, kitti00) and scores the map again with
+    `score_only` when it is 3 (sharded). Counted in the kernels one eager pair launched: one dense_score_kernel (the frontend's) or two."""
     names = gpu_run(name, "eager")["kernels"]
     want = 2 if WORKLOADS[name]["kernel_size"] != 7 else 1
     assert names.count("dense_score_kernel") == want, (name, sorted(set(names)))

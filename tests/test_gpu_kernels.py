@@ -187,9 +187,10 @@ def test_lookup_integer_coords_first_iteration(ops):
 
 
 # ---- (a7) dense post-processing: bit exact ----------------------------------------------------------------
+@pytest.mark.parametrize("name", list(cases.DENSE_CASES))
 @pytest.mark.parametrize("epd", [0, 1])
-def test_dense_postproc_bit_exact(ops, golden, epd):
-    g = golden(f"dense_small_{epd}.pt")
+def test_dense_postproc_bit_exact(ops, golden, epd, name):
+    g = golden(f"dense_{name}_{epd}.pt")
     H, W = g["shape"]
     flow, cov = cases.dense_inputs(H, W)
     out = ops.dense_postproc(flow.to(DEV), cov.to(DEV), 0.25 * 320.0, bool(epd))
@@ -228,17 +229,18 @@ def test_selectors_bit_exact(ops, golden, name):
     d = ops.dense_postproc(flow.to(DEV), cov.to(DEV), 0.25 * 320.0, False, score=score)   # fused scoring
     cand = ops.CandidateList(H, W, DEV)
     mm = cases.selector_match_mask(H, W).to(DEV) if g["variant"] == "masked" else None
-    expect_variants(lambda: ops.select_candidates(score, 32, 100.0, mm, cand), "flag_count_kernel<0>")
+    mw = cases.selector_mask_width(name)
+    expect_variants(lambda: ops.select_candidates(score, mw, 100.0, mm, cand), "flag_count_kernel<0>")
     torch.manual_seed(cases.SELECTOR_RNG_SEED)
     kp = ops.sample_candidates(cand, g["num"])
     mcand = ops.CandidateList(H, W, DEV)
-    expect_variants(lambda: ops.select_mapping_candidates(d["depth"], d["depth_cov"], 32, 5.0, 0.005, mcand), "flag_count_kernel<1>")
+    expect_variants(lambda: ops.select_mapping_candidates(d["depth"], d["depth_cov"], mw, 5.0, 0.005, mcand), "flag_count_kernel<1>")
     mp = ops.sample_candidates(mcand, 2000)
     assert kp.dtype == torch.int64 and kp.is_cuda
     assert torch.equal(kp.cpu(), g["kp"]), "keypoint indices must be bit-exact"
     assert torch.equal(mp.cpu(), g["map_kp"]), "mapping-point indices must be bit-exact"
     # the deterministic half against the oracle: identical candidate mask and threshold
-    mask, thr = okp.candidate_mask_nodepth(ofe.dense_postproc(flow, cov, 0.25, 320.0)["flow_cov"], 7, 32, 100.0,
+    mask, thr = okp.candidate_mask_nodepth(ofe.dense_postproc(flow, cov, 0.25, 320.0)["flow_cov"], 7, mw, 100.0,
                                            cases.selector_match_mask(H, W) if g["variant"] == "masked" else None)
     n = int(cand.n.item())
     assert n == int(mask.sum())
@@ -282,7 +284,8 @@ def test_depth_aware_selector_bit_exact(ops, golden, name):
     mm = cases.selector_match_mask(H, W).to(DEV) if g["variant"] == "masked" else None
     score, cand = ops.ScoreBuffers(H, W, DEV, 7), ops.CandidateList(H, W, DEV)
     ops.score_depth_aware(d1["flow_cov"], d0["depth_cov"], d1["depth_cov"], score)
-    expect_variants(lambda: ops.select_candidates_depth(score, d0["depth"], d1["depth"], d0["depth_cov"], 32, 320.0 * 0.25, 250.0,
+    mw = cases.selector_mask_width(name)
+    expect_variants(lambda: ops.select_candidates_depth(score, d0["depth"], d1["depth"], d0["depth_cov"], mw, 320.0 * 0.25, 250.0,
                                                         100.0, m0, mm, cand), "flag_count_kernel<2>")
     torch.manual_seed(cases.SELECTOR_RNG_SEED)
     kp = ops.sample_candidates(cand, g["num"])
@@ -478,7 +481,8 @@ def test_cov_sanity_filter_kernel(ops):
     assert torch.equal(good, ~bad) and int((~good).sum()) == 4
 
 
-@pytest.mark.parametrize("name", ["depth_small", "depth_masked", "depth_nan"])
+@pytest.mark.parametrize("name", ["depth_small", "depth_masked", "depth_nan", "depth_euroc", "depth_kitti", "depth_kitti00",
+                                  "depth_kitti00_nan", "depth_ragged", "depth_ragged_ties"])
 def test_depth_aware_selector_plugin_class(ops, golden, name):
     """the PLUGIN class `B200_CovAwareSelector` (not just the ops): constructed from a YAML-shaped config with
     `max_depth: auto`, fed `IStereoDepth.Output` / `IMatcher.Output`-shaped objects like MACVO.py does"""
@@ -489,7 +493,8 @@ def test_depth_aware_selector_plugin_class(ops, golden, name):
     (f0, c0), (f1, c1) = cases.selector_depth_inputs(H, W, g["variant"])
     d0 = ops.dense_postproc(f0.to(DEV), c0.to(DEV), 0.25 * 320.0, g["variant"] == "masked")
     d1 = ops.dense_postproc(f1.to(DEV), c1.to(DEV), 0.25 * 320.0, False)
-    cfg = NS(device=DEV, mask_width=32, max_depth="auto", kernel_size=7, max_depth_cov=250.0, max_match_cov=100.0)
+    cfg = NS(device=DEV, mask_width=cases.selector_mask_width(name), max_depth="auto", kernel_size=7, max_depth_cov=250.0,
+             max_match_cov=100.0)
     P.B200_CovAwareSelector.is_valid_config(cfg)
     sel = P.B200_CovAwareSelector(cfg)
     depth0 = NS(depth=d0["depth"], cov=d0["depth_cov"], mask=(~d0["depth_mask"] if g["variant"] == "masked" else None))

@@ -47,9 +47,10 @@ def test_window_lookup_axis_quirk():
     assert torch.allclose(out[4, :], torch.full((9,), 4.0), atol=1e-5)  # j -> y offset (no change on an x-ramp)
 
 
+@pytest.mark.parametrize("name", list(cases.DENSE_CASES))
 @pytest.mark.parametrize("epd", [0, 1])
-def test_dense_postproc(golden, epd):
-    g = golden(f"dense_small_{epd}.pt")
+def test_dense_postproc(golden, epd, name):
+    g = golden(f"dense_{name}_{epd}.pt")
     H, W = g["shape"]
     flow, cov = cases.dense_inputs(H, W)
     out = ofe.dense_postproc(flow, cov, torch.tensor([0.25]).item(), torch.tensor(320.0).item(), bool(epd))
@@ -68,9 +69,10 @@ def test_selectors_bit_exact(golden, name):
     flow, cov = cases.selector_inputs(H, W, g["variant"])
     d = ofe.dense_postproc(flow, cov, 0.25, 320.0)
     mm = cases.selector_match_mask(H, W) if g["variant"] == "masked" else None
+    mw = cases.selector_mask_width(name)
     torch.manual_seed(cases.SELECTOR_RNG_SEED)
-    kp = okp.cov_aware_select_nodepth(d["flow_cov"], g["num"], 7, 32, 100.0, mm)
-    mp = okp.mapping_select(d["depth"], d["depth_cov"], 2000, 5.0, 0.005, 32)
+    kp = okp.cov_aware_select_nodepth(d["flow_cov"], g["num"], 7, mw, 100.0, mm)
+    mp = okp.mapping_select(d["depth"], d["depth_cov"], 2000, 5.0, 0.005, mw)
     assert kp.dtype == torch.int64 and torch.equal(kp, g["kp"])
     assert torch.equal(mp, g["map_kp"])
 
@@ -91,7 +93,7 @@ def test_depth_aware_selector_bit_exact(golden, name):
     d0, d1, m0, mm = _depth_selector_inputs(g)
     torch.manual_seed(cases.SELECTOR_RNG_SEED)
     kp = okp.cov_aware_select(d1["flow_cov"], d0["depth"], d0["depth_cov"], d1["depth"], d1["depth_cov"], g["num"],
-                              7, 32, 320.0 * 0.25, 250.0, 100.0, m0, mm)
+                              7, cases.selector_mask_width(name), 320.0 * 0.25, 250.0, 100.0, m0, mm)
     assert torch.equal(kp, g["kp"])
 
 

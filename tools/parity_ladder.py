@@ -1,8 +1,10 @@
-"""Per-stage error ladder of the FlowFormerCov frontend at 640x480 / decoder_depth 12 (BASELINE configs[1] shape):
-GPU network (strict fp32, and the TF32 / fp16-GMA mode bench.py times) against the float64 ground truth of
-tests/golden/net_cfgA.pt, next to the reference's own fp32 distance from that truth (the noise floor).
+"""Per-stage error ladder of the FlowFormerCov frontend at decoder_depth 12: GPU network (strict fp32, and the TF32 /
+fp16-GMA mode bench.py times) against the float64 ground truth of tests/golden/net_<case>.pt, next to the reference's own
+fp32 distance from that truth (the noise floor). Cases (tests/golden/cases.py::LADDER_CASES): cfgA (640x480, BASELINE
+configs[1] shape), euroc (752x480), kitti (1241x376), kitti00 (1226x370).
 
     python tools/parity_ladder.py [--out gpurun_out/parity_ladder.json]
+    python tools/parity_ladder.py --case kitti --out <file>.json      (another frame size)
 
 Error measure per stage: max |x - truth| / mean |truth|  (relative to the stage's scale); covariance: max relative.
 """
@@ -29,15 +31,16 @@ def set_mode(mode: str) -> None:
     torch.set_float32_matmul_precision("medium" if tf32 else "highest")
 
 
-def ladder(mode: str, golden: dict, device: str = "cuda") -> dict:
+def ladder(mode: str, golden: dict, case: str = "cfgA", device: str = "cuda") -> dict:
     from macvo_b200.flowformer_cov import FlowFormerCovNet, synthetic_state_dict
     set_mode(mode)
-    A, B = cases.cfgA_inputs()
+    A, B = cases.ladder_inputs(case)
+    assert golden["shape"] == (2, *cases.LADDER_CASES[case]), (golden["shape"], case)
     net = FlowFormerCovNet(synthetic_state_dict(0), device, decoder_depth=golden["decoder_depth"])
     net.taps = {}
     flow, cov = net.inference(A.to(device), B.to(device))
     torch.cuda.synchronize()
-    T, S = golden["truth"], cases.cfgA_sample
+    T, S = golden["truth"], (lambda name, t: cases.ladder_sample(case, name, t))
     rel = lambda x, t: ((x.double().cpu() - t).abs().max() / t.abs().mean()).item()
     out = {}
     for name in STAGES:
@@ -57,15 +60,16 @@ def ladder(mode: str, golden: dict, device: str = "cuda") -> dict:
 
 def main() -> None:
     ap = argparse.ArgumentParser()
+    ap.add_argument("--case", default="cfgA", choices=list(cases.LADDER_CASES))
     ap.add_argument("--out", default=os.path.join(REPO, "gpurun_out", "parity_ladder.json"))
     a = ap.parse_args()
-    g = torch.load(os.path.join(REPO, "tests", "golden", "net_cfgA.pt"), weights_only=False)
+    g = torch.load(os.path.join(REPO, "tests", "golden", f"net_{a.case}.pt"), weights_only=False)
     T, r = g["truth"], g["ref32"]
     floor = {"flow": ((r["flow"].double() - T["flow"]).abs().max() / T["flow"].abs().mean()).item(),
              "cov_rel_max": ((r["cov"].double() - T["cov"]).abs() / T["cov"].abs()).max().item()}
-    res = {"floor_ref32_vs_truth": floor, "floor_full_tensor": g["floor"]}
+    res = {"case": a.case, "floor_ref32_vs_truth": floor, "floor_full_tensor": g["floor"]}
     for mode in ("strict", "tf32"):
-        res[mode] = ladder(mode, g)
+        res[mode] = ladder(mode, g, a.case)
     os.makedirs(os.path.dirname(a.out), exist_ok=True)
     json.dump(res, open(a.out, "w"), indent=1)
     print(f"{'stage':<14}{'strict fp32':>14}{'tf32 mode':>14}")
