@@ -41,7 +41,7 @@ def window_lookup(cost_maps: Tensor, coords: Tensor) -> Tensor:
     but adds it to (x, y), so the FIRST window axis steps in x. Output channel = i*9 + j.
     """
     B, _, H1, W1 = coords.shape
-    r = torch.linspace(-4, 4, 9, dtype=coords.dtype)
+    r = torch.linspace(-4, 4, 9, dtype=coords.dtype, device=coords.device)
     delta = torch.stack(torch.meshgrid(r, r, indexing="ij"), dim=-1).view(1, 9, 9, 2)
     c = coords.permute(0, 2, 3, 1).reshape(B * H1 * W1, 1, 1, 2) + delta
     H2, W2 = cost_maps.shape[-2:]

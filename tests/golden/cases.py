@@ -320,17 +320,96 @@ def _typed_fields(c: dict) -> dict:
             "pts_cov": c["pts_cov"].double().numpy()}
 
 
+# ---- sharpened checkpoint -----------------------------------------------------------------------------------------------
+# `synthetic_state_dict(0)` draws every weight from U(+-1/sqrt(fan_in)): its attention logits have a std of 0.02 - 0.6
+# and every softmax of the frontend is close to uniform, so the network's output is close to the mean of the values and
+# an error in how the network calls its attention kernels (scale, key / value pairing, position terms) shrinks by one to
+# two orders of magnitude before it reaches the flow. The sharpened checkpoint multiplies the query and key projections
+# (weight and bias rows) of every softmax family by a power of two, which is exact in fp32 and under tf32 / fp16
+# rounding. Gains per family: (query gain, key gain); the mask families scale the 576-channel logit convolution itself.
+# Chosen by tests/golden/make_golden_sharp.py::calibrate for a median logit std in [2, 4] per family (float64, 640x480,
+# decoder_depth 3); the GRU gates are not scaled (saturated gates only lower the sensitivity and raise the fp32 noise).
+SHARP_GAINS = {"svt_local": (8.0, 4.0), "svt_global": (8.0, 4.0), "perceiver_input": (8.0, 4.0), "latent": (4.0, 2.0),
+               "vert_local": (4.0, 4.0), "vert_global": (4.0, 2.0), "cross_attend": (2.0, 2.0), "gma": (16.0, 8.0),
+               "mask_flow": 64.0, "mask_cov": 64.0}
+# the median logit std every family of the sharpened checkpoint reaches (make_golden_sharp.py asserts it per fixture)
+SHARP_TARGET = (2.0, 4.0)
+
+
+def sharp_rows() -> dict[str, list[tuple[int, int, str, int]]]:
+    """checkpoint key -> [(first row, end row, family, 0 = query gain / 1 = key gain), ...] of every scaled tensor"""
+    out: dict[str, list[tuple[int, int, str, int]]] = {}
+
+    def add(key: str, lo: int, hi: int, fam: str, which: int) -> None:
+        for t in ("weight", "bias"):
+            out.setdefault(f"{key}.{t}", []).append((lo, hi, fam, which))
+    for enc in ("memory_encoder.feat_encoder", "context_encoder"):
+        for s, C in enumerate((128, 256)):
+            b = f"{enc}.svt.blocks.{s}."
+            add(b + "0.attn.qkv", 0, C, "svt_local", 0)                  # rows [q | k | v]
+            add(b + "0.attn.qkv", C, 2 * C, "svt_local", 1)
+            add(b + "1.attn.q", 0, C, "svt_global", 0)
+            add(b + "1.attn.kv", 0, C, "svt_global", 1)                   # rows [k | v]
+    c = "memory_encoder.cost_perceiver_encoder."
+    layers = [(c + "input_layer.", "perceiver_input")] + [(c + f"encoder_layers.{i}.", "latent") for i in range(3)]
+    for i in range(3):
+        layers += [(c + f"vertical_encoder_layers.{i}.local_block.attn.", "vert_local"),
+                   (c + f"vertical_encoder_layers.{i}.global_block.attn.", "vert_global")]
+    layers += [("memory_decoder.decoder_layer.cross_attend.", "cross_attend")]
+    for p, fam in layers:
+        add(p + "q", 0, 128 if fam != "cross_attend" else 64, fam, 0)
+        add(p + "k", 0, 128 if fam != "cross_attend" else 64, fam, 1)
+    out["memory_decoder.att.to_qk.weight"] = [(0, 128, "gma", 0), (128, 256, "gma", 1)]    # no bias
+    for p, fam in (("memory_decoder.update_block.", "mask_flow"), ("memory_decoder.cov_update.", "mask_cov")):
+        add(p + "mask.2", 0, 576, fam, 0)
+    return out
+
+
+def sharp_gain(gains: dict, fam: str, which: int) -> float:
+    g = gains[fam]
+    return float(g) if not isinstance(g, tuple) else float(g[which])
+
+
+def sharp_state_dict(gains: dict | None = None) -> dict[str, Tensor]:
+    """`synthetic_state_dict(0)` with the query / key rows of every softmax family times its power-of-two gain
+    (`SHARP_GAINS`, or `gains` during calibration)"""
+    from macvo_b200.flowformer_cov import synthetic_state_dict
+    gains = SHARP_GAINS if gains is None else gains
+    sd = synthetic_state_dict(0)
+    for key, rows in sharp_rows().items():
+        t = sd[key].clone()
+        for lo, hi, fam, which in rows:
+            t[lo:hi] *= sharp_gain(gains, fam, which)
+        sd[key] = t
+    return sd
+
+
+def ladder_state_dict(weights: str) -> dict[str, Tensor]:
+    """the checkpoint a parity fixture records in its `weights` entry: "synthetic:<seed>" or "sharp:0" """
+    kind, seed = weights.split(":")
+    if kind == "synthetic":
+        from macvo_b200.flowformer_cov import synthetic_state_dict
+        return synthetic_state_dict(int(seed))
+    if kind == "sharp" and seed == "0":
+        return sharp_state_dict()
+    raise ValueError(f"unknown weights {weights!r}")
+
+
 # ---- depth-12 network parity ladder: 640x480 (BASELINE configs[1] shape) and the shipped dataset frame sizes ----------
 # (H, W) of the frame. cfgA and TartanAir share 640x480; EuRoC is 752x480 (1/8 grid 60x94); KITTI is 1241x376 (padded
-# to 1248x376, 1/8 grid 47x156) and 1226x370 for sequences 00-02 (padded to 1232x376, 1/8 grid 47x154).
-LADDER_CASES = {"cfgA": (480, 640), "euroc": (480, 752), "kitti": (376, 1241), "kitti00": (370, 1226)}
+# to 1248x376, 1/8 grid 47x156) and 1226x370 for sequences 00-02 (padded to 1232x376, 1/8 grid 47x154). The sharp cases
+# run the sharpened checkpoint (`LADDER_WEIGHTS`) on the cfgA and kitti00 frames.
+LADDER_CASES = {"cfgA": (480, 640), "euroc": (480, 752), "kitti": (376, 1241), "kitti00": (370, 1226),
+                "sharp": (480, 640), "sharp_kitti00": (370, 1226)}
+LADDER_WEIGHTS = {"sharp": "sharp:0", "sharp_kitti00": "sharp:0"}       # every other case: "synthetic:0"
 # strided samples of each stage, the same indices on both sides of the comparison: full-resolution pixel stride (phase
 # 2; 5 and 21 are coprime with 8, so every 8x8 upsampling phase is sampled), feature (channel, row, column) strides,
 # correlation (tapped row, column) strides, cost-memory (row, channel) strides and the 1/8-grid iterate stride. Coarser at
 # the dataset sizes, so that each of their fixtures stays under 0.5 MB.
 _DATASET_SAMPLE = {"px": 21, "feat": (32, 8, 14), "corr": (10, 35), "mem": (388, 8), "iter": 6}
 _LADDER_SAMPLES = {"cfgA": {"px": 5, "feat": (8, 4, 5), "corr": (5, 7), "mem": (37, 4), "iter": 2},
-                   "euroc": _DATASET_SAMPLE, "kitti": _DATASET_SAMPLE, "kitti00": _DATASET_SAMPLE}
+                   "euroc": _DATASET_SAMPLE, "kitti": _DATASET_SAMPLE, "kitti00": _DATASET_SAMPLE,
+                   "sharp": _DATASET_SAMPLE, "sharp_kitti00": _DATASET_SAMPLE}
 
 
 def ladder_inputs(case: str = "cfgA") -> tuple[Tensor, Tensor]:

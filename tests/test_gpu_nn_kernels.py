@@ -75,6 +75,41 @@ ATTN_CASES = [(37, 8, 80, 8, 16, True), (50, 8, 8, 8, 16, False), (33, 1, 8, 8, 
               (2, 700, 300, 4, 32, False), (2, 130, 75, 8, 32, False), (1, 5, 513, 8, 16, False),
               (5, 6, 21, 4, 32, False), (7, 3, 10, 8, 16, False), (2, 9, 30, 8, 16, False),
               (41, 1, 8, 8, 8, False), (6, 8, 20, 8, 8, True), (77, 1, 8, 4, 16, False), (300, 1, 5, 8, 8, False)]
+# the same shapes with "peaked" inputs (`_plant_dominant_key`): one key 30 above the rest of its row's logits, last in one
+# row and first in another. Placed last, it arrives in the final (mostly partial) key chunk, so the running maximum of the
+# online softmax changes at the very end and the whole accumulator has to be rescaled by exp(-30 - ...) there.
+ATTN_CASES += [c + ("peaked",) for c in ATTN_CASES]
+
+
+def _plant_dominant_key(q, k, heads, bc):
+    """in place: in every head, key nk-1 of batch 0 outscores the other keys of query row 0 by 30, and key 0 of the last
+    batch those of query row nq-1 (a different row, or a different batch when nq = 1). Each planted key is the query it
+    serves with the other planted row's query projected out, so it moves no other logit of those two rows; the margin
+    is asserted on the float64 logits."""
+    B, nk, C = k.shape
+    d = C // heads
+    nq = q.shape[1]
+    plant = ((0, 0, nk - 1), (B - 1, nq - 1, 0))
+    qrow = lambda b, i: q[0 if bc else b, i].double().view(heads, d)
+    logits = lambda b, i: torch.einsum("hd,jhd->hj", qrow(b, i), k[b].double().view(nk, heads, d)) * d ** -0.5
+    for b, _, j in plant:
+        k[b, j] = 0.0
+    new = []
+    for n, (b, i, j) in enumerate(plant):
+        qi, (bo, io, _) = qrow(b, i), plant[1 - n]
+        if bo == b:
+            qo = qrow(bo, io)
+            qi = qi - ((qi * qo).sum(1) / (qo * qo).sum(1))[:, None] * qo
+        lg = logits(b, i)
+        others = torch.cat([lg[:, :j], lg[:, j + 1:]], 1).amax(1)
+        scale = (others + 30.0) * d ** 0.5 / (qi * qrow(b, i)).sum(1)      # logit of the new key j = others + 30
+        new.append(qi * scale[:, None])
+    for (b, _, j), kj in zip(plant, new):
+        k[b, j] = kj.view(C).to(k.dtype)
+    for b, i, j in plant:
+        lg = logits(b, i)
+        others = torch.cat([lg[:, :j], lg[:, j + 1:]], 1).amax(1)
+        assert (lg[:, j] - others).min().item() >= 29.99
 
 
 def _attn_variant(b, nq, heads, d, bc, tf32):
@@ -89,11 +124,14 @@ def _attn_variant(b, nq, heads, d, bc, tf32):
 
 @pytest.mark.parametrize("case", ATTN_CASES)
 def test_small_attention(ops, case):
-    b, nq, nk, heads, d, bc = case
+    b, nq, nk, heads, d, bc, *mode = case
     g = torch.Generator().manual_seed(sum(case[:5]))
-    q = (torch.randn(1 if bc else b, nq, heads * d, generator=g) * 1.5).to(DEV)
-    k = (torch.randn(b, nk, heads * d, generator=g) * 1.5).to(DEV)
-    v = torch.randn(b, nk, heads * d, generator=g).to(DEV)
+    q = torch.randn(1 if bc else b, nq, heads * d, generator=g) * 1.5
+    k = torch.randn(b, nk, heads * d, generator=g) * 1.5
+    v = torch.randn(b, nk, heads * d, generator=g)
+    if mode == ["peaked"]:
+        _plant_dominant_key(q, k, heads, bc)
+    q, k, v = q.to(DEV), k.to(DEV), v.to(DEV)
     ref = _ref_attention(q, k, v, heads)
     got = expect_variants(lambda: ops.small_attention(q, k, v, heads, allow_tf32=False), _attn_variant(b, nq, heads, d, bc, False))
     assert got.shape == ref.shape
@@ -221,6 +259,15 @@ def test_softmax_rows_f16(ops, rows, cols):
     assert got.dtype == torch.float16 and got.shape == x.shape
     assert ((got.double() - ref).abs() <= ref * 2.0 ** -10 + 1e-7).all()
     assert (got.double().sum(-1) - 1).abs().max().item() <= 2e-3
+    # peaked rows: one logit 30 above the rest of its row, last in row 0 (the final partial quad when cols % 8 = 4) and
+    # first in the last row; every other weight of those rows is below exp(-30) and must come out as 0 or a subnormal
+    p = (torch.randn(rows, cols, generator=g) * 6).to(DEV)
+    p[0, -1] = p[0, :-1].max() + 30.0
+    p[-1, 0] = p[-1, 1:].max() + 30.0
+    got = ops.softmax_rows_f16(p)
+    ref = torch.softmax(p.double(), dim=-1)
+    assert ((got.double() - ref).abs() <= ref * 2.0 ** -10 + 1e-7).all()
+    assert got[0, -1].item() == 1.0 and got[-1, 0].item() == 1.0
     with pytest.raises(ops.MacvoB200Error):
         ops.softmax_rows_f16(x.cpu())
 

@@ -27,6 +27,20 @@ for the flow by any faithful fp32 implementation and is AT the fp32 noise floor 
            the encoders already differ by 3.5e-3 of their scale, the refinement contracts that to 6e-4 on the flow.
            Bounds = 1.5 x the measured ladder (tools/parity_ladder.py), so that one dropped mantissa bit
            (2 x the error) fails the test.
+
+sharp, sharp_kitti00: the sharpened checkpoint (tests/golden/cases.py::sharp_state_dict) on the cfgA and kitti00 frames
+and branches. With the synthetic checkpoint every softmax is close to uniform, so an error in the plumbing around the
+attention kernels (a scale, which keys go with which values, a position term) shrinks by one to two orders of magnitude
+before it reaches the flow; with the sharpened one every family's median logit std is 2 - 4 (recorded in the fixture).
+Sharper softmaxes also amplify rounding, so these cases are held to their own yardsticks where those are looser:
+  strict   every stage within max(BOUNDS strict, 3 x the fixture's fp32 noise floor of that stage: the same class in fp32
+           on the CPU against the float64 truth), plus the 2.5 x floor rule on the final flow and covariance;
+  tf32     every stage within max(BOUNDS tf32, 1.5 x the library-op path's error at that stage, measured in the same
+           test: the same class with none of our kernels, torch / cuDNN / cuBLAS ops under the same TF32 flags, as the
+           reference runs on a GPU); 2 x for the full-resolution outputs. The convex upsampling's 64x sharper mask
+           amplifies the rounding of the last state, so the two faithful TF32 runs differ more there than anywhere on the
+           1/8 grid: on an H100 80GB HBM3 (700 W) our flow error was 0.84x (sharp) and 1.59x (sharp_kitti00) the library
+           path's while every 1/8-grid iterate stayed within 1.12x; a GMA temperature error still exceeds the bound 20x.
 """
 import os
 import sys
@@ -52,11 +66,13 @@ BOUNDS = {
 # flow_vs_ref32 / cov_rel_vs_ref32 (the distance to the reference's fp32 output).
 
 
-LADDER_CASES = ("cfgA", "euroc", "kitti", "kitti00")
+LADDER_CASES = ("cfgA", "euroc", "kitti", "kitti00", "sharp", "sharp_kitti00")
+SHARP_CASES = ("sharp", "sharp_kitti00")
+FULL_RESOLUTION = ("flow", "cov_rel_max", "flow_vs_ref32", "cov_rel_vs_ref32")      # after the convex upsampling
 # which branch each dispatch point takes, per case (the table above): correlation mode in TF32 mode (strict: the fp32-class
 # 3 x fp16 split wherever TF32 takes the tensor cores), whether the fp16 GMA softmax kernel runs, native vertical attention
 BRANCHES = {"cfgA": ("tf32", True, True), "euroc": ("tf32", True, False), "kitti": ("simt", True, False),
-            "kitti00": ("simt", False, False)}
+            "kitti00": ("simt", False, False), "sharp": ("tf32", True, True), "sharp_kitti00": ("simt", False, False)}
 
 
 @pytest.fixture(scope="module")
@@ -107,21 +123,33 @@ def test_frontend_parity_ladder(ladder_fn, golden, monkeypatch, mode, case):
     g = golden(f"net_{case}.pt")
     rec = _record_branches(monkeypatch)
     prev = (torch.backends.cuda.matmul.allow_tf32, torch.backends.cudnn.allow_tf32, torch.get_float32_matmul_precision())
+    lib = None
     try:
+        if case in SHARP_CASES and mode == "tf32":
+            lib = ladder_fn.ladder(mode, g, case, library_ops=True)
+            rec.update(corr=[], softmax_f16=0, vglobal=0, vglobal_native=0)
         res = ladder_fn.ladder(mode, g, case)
     finally:
         torch.backends.cuda.matmul.allow_tf32, torch.backends.cudnn.allow_tf32 = prev[0], prev[1]
         torch.set_float32_matmul_precision(prev[2])
     col = 0 if mode == "strict" else 1
-    bound = {name: b[col] for name, b in BOUNDS.items()}
-    report = []
-    for name in BOUNDS:
-        val = max(res[name]) if isinstance(res[name], list) else res[name]
-        report.append(f"{name} {val:.3e} (bound {bound[name]:.2e})")
+    # per stage (per iteration for the iterates): the fixed bound, or for the sharp cases the larger of it and the case's
+    # own yardstick (module docstring)
+    yard, mult = (g.get("floor_stages"), 3.0) if mode == "strict" else (lib, 1.5)
+    as_list = lambda v: v if isinstance(v, list) else [v]
+    bound = {}
+    for name, b in BOUNDS.items():
+        n = len(as_list(res[name]))
+        m = 2.0 if mode == "tf32" and name in FULL_RESOLUTION else mult
+        bound[name] = [max(b[col], m * y) for y in as_list(yard[name])] if case in SHARP_CASES else [b[col]] * n
+        assert len(bound[name]) == n, (name, n)
+    report = [f"{name} {max(as_list(res[name])):.3e} (bound {max(bound[name]):.2e})" for name in BOUNDS]
     print(f"[{case} {mode}] " + "; ".join(report))
+    if lib is not None:
+        print(f"[{case} {mode} library ops] " + "; ".join(f"{name} {max(as_list(lib[name])):.3e}" for name in BOUNDS))
     for name in BOUNDS:
-        val = max(res[name]) if isinstance(res[name], list) else res[name]
-        assert val <= bound[name], f"{case} {mode}: stage {name}: {val:.3e} > {bound[name]:.2e}  | full ladder: {report}"
+        for i, (val, b) in enumerate(zip(as_list(res[name]), bound[name])):
+            assert val <= b, f"{case} {mode}: stage {name}[{i}]: {val:.3e} > {b:.2e}  | full ladder: {report}"
     if mode == "strict":
         floor = g["floor"]
         assert res["flow_abs_max"] <= 2.5 * floor["flow_abs_max"] and res["cov_rel_max"] <= 2.5 * floor["cov_rel_max"]

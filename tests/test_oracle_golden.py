@@ -191,6 +191,42 @@ def test_cfgA_fixture_records_the_fp32_noise_floor(golden):
     assert len(g["truth"]["flow_iter"]) == 12 and g["truth"]["flow"].dtype == torch.float64
 
 
+def test_sharp_checkpoint_and_fixtures_reach_their_regime(golden):
+    """cases.sharp_state_dict differs from synthetic_state_dict(0) in the listed query / key rows only, each by its family's
+    power-of-two gain (exact in fp32); net_sharp*.pt were made from it, and every softmax family reached a median logit
+    std in cases.SHARP_TARGET on the fixture's own frames, with fp32 noise floors recorded for every ladder stage."""
+    import math
+    from macvo_b200.flowformer_cov import synthetic_state_dict
+    base, sharp, rows = synthetic_state_dict(0), cases.sharp_state_dict(), cases.sharp_rows()
+    assert base.keys() == sharp.keys()
+    families = set()
+    for key, t in base.items():
+        expect = t.clone()
+        for lo, hi, fam, which in rows.get(key, []):
+            g = cases.sharp_gain(cases.SHARP_GAINS, fam, which)
+            assert math.frexp(g)[0] == 0.5 and g > 1, (key, g)          # a power of two above 1
+            expect[lo:hi] *= g
+            families.add(fam)
+        assert torch.equal(sharp[key], expect), key                       # bit for bit, every other row / tensor unchanged
+    assert families == set(cases.SHARP_GAINS)
+    assert not any(".gru." in k for k in rows)                           # the GRU gates keep their weights
+    lo, hi = cases.SHARP_TARGET
+    cfgA = golden("net_cfgA.pt")["floor"]
+    for case, weights in cases.LADDER_WEIGHTS.items():
+        g = golden(f"net_{case}.pt")
+        assert g["weights"] == weights == "sharp:0" and g["shape"] == (2, *cases.LADDER_CASES[case])
+        assert set(g["regime"]) == families
+        for fam, st in g["regime"].items():
+            assert lo <= st["logit_std_median"] <= hi, (case, fam, st)
+            assert 1.0 / st["keys"] < st["max_weight_median"] <= 1.0, (case, fam, st)
+        fl = g["floor"]
+        assert fl["flow_abs_max"] / fl["flow_scale"] <= 10 * cfgA["flow_abs_max"] / cfgA["flow_scale"]
+        assert fl["cov_rel_max"] <= 10 * cfgA["cov_rel_max"]
+        stages = g["floor_stages"]
+        assert len(stages["flow_iter"]) == len(stages["cov_iter"]) == 12 == len(g["truth"]["flow_iter"])
+        assert all(0 < v < 1e-3 for v in stages["flow_iter"] + stages["cov_iter"] + [stages["flow"], stages["feats"]])
+
+
 def test_golden_inputs_reproduce_bit_for_bit(golden):
     """Every fixture records the sha256 of the seeded inputs it was generated from; the generators (tests/golden/cases.py)
     use exactly rounded operations only, so this host must regenerate the same bits. Regression test of the round-1

@@ -1,7 +1,12 @@
 """Per-stage error ladder of the FlowFormerCov frontend at decoder_depth 12: GPU network (strict fp32, and the TF32 /
 fp16-GMA mode bench.py times) against the float64 ground truth of tests/golden/net_<case>.pt, next to the reference's own
 fp32 distance from that truth (the noise floor). Cases (tests/golden/cases.py::LADDER_CASES): cfgA (640x480, BASELINE
-configs[1] shape), euroc (752x480), kitti (1241x376), kitti00 (1226x370).
+configs[1] shape), euroc (752x480), kitti (1241x376), kitti00 (1226x370), and sharp / sharp_kitti00 (the sharpened
+checkpoint, cases.sharp_state_dict, on the cfgA / kitti00 frames). The network is built from the fixture's `weights`.
+
+`library_ops=True` runs the library-op path instead: the same class with none of our kernels (`_ops = None`: torch /
+cuDNN / cuBLAS ops, the oracle's correlation and window lookup) on the device under the same precision flags — what the
+reference itself runs on a GPU, and the yardstick of the sharp cases in TF32 mode.
 
     python tools/parity_ladder.py [--out gpurun_out/parity_ladder.json]
     python tools/parity_ladder.py --case kitti --out <file>.json      (another frame size)
@@ -31,12 +36,17 @@ def set_mode(mode: str) -> None:
     torch.set_float32_matmul_precision("medium" if tf32 else "highest")
 
 
-def ladder(mode: str, golden: dict, case: str = "cfgA", device: str = "cuda") -> dict:
+def ladder(mode: str, golden: dict, case: str = "cfgA", device: str = "cuda", library_ops: bool = False) -> dict:
     from macvo_b200.flowformer_cov import FlowFormerCovNet, synthetic_state_dict
+    from oracle import frontend as ofe
     set_mode(mode)
     A, B = cases.ladder_inputs(case)
     assert golden["shape"] == (2, *cases.LADDER_CASES[case]), (golden["shape"], case)
-    net = FlowFormerCovNet(synthetic_state_dict(0), device, decoder_depth=golden["decoder_depth"])
+    weights = golden.get("weights", "synthetic:0")          # fixtures without the entry were made from synthetic:0
+    sd = synthetic_state_dict(0) if weights == "synthetic:0" else cases.ladder_state_dict(weights)
+    net = FlowFormerCovNet(sd, device, decoder_depth=golden["decoder_depth"])
+    if library_ops:
+        net._ops, net.corr_fn, net.lookup_fn = None, ofe.corr_volume, ofe.window_lookup
     net.taps = {}
     flow, cov = net.inference(A.to(device), B.to(device))
     torch.cuda.synchronize()
@@ -68,18 +78,20 @@ def main() -> None:
     floor = {"flow": ((r["flow"].double() - T["flow"]).abs().max() / T["flow"].abs().mean()).item(),
              "cov_rel_max": ((r["cov"].double() - T["cov"]).abs() / T["cov"].abs()).max().item()}
     res = {"case": a.case, "floor_ref32_vs_truth": floor, "floor_full_tensor": g["floor"]}
+    cols = ("strict", "tf32", "lib_tf32")
     for mode in ("strict", "tf32"):
         res[mode] = ladder(mode, g, a.case)
+    res["lib_tf32"] = ladder("tf32", g, a.case, library_ops=True)
     os.makedirs(os.path.dirname(a.out), exist_ok=True)
     json.dump(res, open(a.out, "w"), indent=1)
-    print(f"{'stage':<14}{'strict fp32':>14}{'tf32 mode':>14}")
+    print(f"{'stage':<18}" + "".join(f"{c:>12}" for c in cols))
     for name in STAGES:
-        print(f"{name:<14}{res['strict'][name]:>14.3e}{res['tf32'][name]:>14.3e}")
-    for i in range(len(res["strict"]["flow_iter"])):
-        print(f"flow iter {i + 1:<4}{res['strict']['flow_iter'][i]:>14.3e}{res['tf32']['flow_iter'][i]:>14.3e}"
-              f"   cov iter {res['strict']['cov_iter'][i]:>10.3e}{res['tf32']['cov_iter'][i]:>12.3e}")
+        print(f"{name:<18}" + "".join(f"{res[c][name]:>12.3e}" for c in cols))
+    for it in ("flow_iter", "cov_iter"):
+        for i in range(len(res["strict"][it])):
+            print(f"{it} {i + 1:<8}" + "".join(f"{res[c][it][i]:>12.3e}" for c in cols))
     for name in ("flow", "flow_abs_max", "cov_rel_max", "cov_rel_p99", "flow_vs_ref32", "cov_rel_vs_ref32"):
-        print(f"{name:<14}{res['strict'][name]:>14.3e}{res['tf32'][name]:>14.3e}")
+        print(f"{name:<18}" + "".join(f"{res[c][name]:>12.3e}" for c in cols))
     print("reference fp32 vs truth (noise floor):", floor)
 
 
