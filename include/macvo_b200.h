@@ -280,6 +280,14 @@ int macvo_pgo_solve_sharded(const double* pos_Tw, const double* kp2_uv, const do
 int macvo_pgo_accumulate(const double* pos_Tw, const double* kp2_uv, const double* kp2_disp, const double* uv_cov,
                          const double* disp_cov, int k, const double* intr, const double* pose, double huber_delta,
                          double* acc, void* stream);
+/* The same accumulator for any graph type (graph_type and the icp columns as in macvo_pgo_solve_graph), reduced over a
+ * cluster of `cluster` CTAs (1..8; 0 = choose from k as the solve does). singular_flag (one device double, may be NULL)
+ * is set to 1 when a covariance block lost an eigenvalue to the pseudo-inverse, like stats[7] of the solve; it is never
+ * cleared. macvo_pgo_accumulate = graph type MACVO_PGO_DISP, cluster 1, no flag. */
+int macvo_pgo_accumulate_graph(int graph_type, const double* pos_Tw, const double* kp2_uv, const double* kp2_disp,
+                               const double* uv_cov, const double* disp_cov, const double* pc_obs, const double* obs_cov,
+                               const double* pts_cov, int k, const double* intr, const double* pose, double huber_delta,
+                               int cluster, double* acc, double* singular_flag, void* stream);
 
 /* ---- frontend "next" rows (SURVEY.md §8f-1/2): memory-bound layers of the cost perceiver ----------------
  * fp32 only; replace the torch ops of Module/Network/FlowFormer/core/encoder.py:12-55 (PatchEmbed conv1 + pad),

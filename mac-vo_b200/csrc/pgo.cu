@@ -66,6 +66,61 @@ __device__ __forceinline__ double huber(double x, double delta) {        // on t
     return s < delta ? x : 2.0 * delta * s - delta * delta;
 }
 
+// torch.pinverse / np.linalg.pinv keep the singular values above this fraction of the largest one
+constexpr double PINV_RCOND = 1e-15;
+
+// one Jacobi rotation of the symmetric 3x3 `a` that zeroes a[p][q] (r is the third index); v accumulates the rotations
+__device__ __forceinline__ void jacobi_rotate(double (&a)[3][3], double (&v)[3][3], int p, int q, int r) {
+    const double apq = a[p][q];
+    if (apq == 0.0) return;
+    const double g = 100.0 * fabs(apq), app = a[p][p], aqq = a[q][q], h = aqq - app;
+    if (fabs(app) + g == fabs(app) && fabs(aqq) + g == fabs(aqq)) { a[p][q] = a[q][p] = 0.0; return; }   // below rounding
+    double t;
+    if (fabs(h) + g == fabs(h)) t = apq / h;
+    else {
+        const double th = 0.5 * h / apq;
+        t = 1.0 / (fabs(th) + sqrt(th * th + 1.0));
+        if (th < 0.0) t = -t;
+    }
+    const double c = 1.0 / sqrt(t * t + 1.0), s = t * c, tau = s / (1.0 + c);
+    a[p][p] = app - t * apq; a[q][q] = aqq + t * apq; a[p][q] = a[q][p] = 0.0;
+    const double arp = a[r][p], arq = a[r][q];
+    a[r][p] = a[p][r] = arp - s * (arq + arp * tau);
+    a[r][q] = a[q][r] = arq + s * (arp - arq * tau);
+#pragma unroll
+    for (int i = 0; i < 3; ++i) {
+        const double vp = v[i][p], vq = v[i][q];
+        v[i][p] = vp - s * (vq + vp * tau);
+        v[i][q] = vq + s * (vp - vq * tau);
+    }
+}
+
+// Moore-Penrose inverse of the symmetric 3x3 [[m00 m01 m02] [. m11 m12] [. . m22]] by cyclic Jacobi: sum of v v^T / lambda
+// over the eigenvalues with |lambda| > PINV_RCOND * max |lambda| (torch.pinverse of a symmetric matrix). Returns true when an
+// eigenvalue was dropped.
+__device__ bool sym3_pinv(double m00, double m01, double m02, double m11, double m12, double m22,
+                          double& w00, double& w01, double& w02, double& w11, double& w12, double& w22) {
+    double a[3][3] = {{m00, m01, m02}, {m01, m11, m12}, {m02, m12, m22}};
+    double v[3][3] = {{1.0, 0.0, 0.0}, {0.0, 1.0, 0.0}, {0.0, 0.0, 1.0}};
+    for (int sweep = 0; sweep < 32 && (a[0][1] != 0.0 || a[0][2] != 0.0 || a[1][2] != 0.0); ++sweep) {
+        jacobi_rotate(a, v, 0, 1, 2);
+        jacobi_rotate(a, v, 0, 2, 1);
+        jacobi_rotate(a, v, 1, 2, 0);
+    }
+    const double lmax = fmax(fabs(a[0][0]), fmax(fabs(a[1][1]), fabs(a[2][2])));
+    w00 = w01 = w02 = w11 = w12 = w22 = 0.0;
+    bool dropped = false;
+#pragma unroll
+    for (int e = 0; e < 3; ++e) {
+        const double l = a[e][e];
+        if (!(fabs(l) > PINV_RCOND * lmax)) { dropped = true; continue; }
+        const double il = 1.0 / l, x = v[0][e], y = v[1][e], z = v[2][e];
+        w00 += x * x * il; w01 += x * y * il; w02 += x * z * il;
+        w11 += y * y * il; w12 += y * z * il; w22 += z * z * il;
+    }
+    return dropped;
+}
+
 __device__ __forceinline__ int tri_index(int e, int& i, int& j) {        // upper-triangular (i <= j) of a 6x6, row-major
     int row = 0, rem = e;
     while (rem >= 6 - row) { rem -= 6 - row; ++row; }
@@ -188,17 +243,22 @@ __device__ void accumulate_full(const Problem& P, const double* posevec, Shared&
             for (int i = 0; i < 3; ++i)
                 for (int j = 0; j < 3; ++j)
                     M[3 * i + j] = RS[3 * i] * S.Rm[3 * j] + RS[3 * i + 1] * S.Rm[3 * j + 1] + RS[3 * i + 2] * S.Rm[3 * j + 2] + Sp[3 * i + j];
-            // inverse of the (symmetrised) 3x3 by cofactors; torch.pinverse == inverse for the positive-definite blocks of this
-            // path; a singular block gets zero weight and is flagged
+            // torch.pinverse of the (symmetrised) 3x3. A positive-definite block takes the cofactor inverse while that is
+            // accurate: det rounds to within a few eps * tr^3, so det >= 1e-6 tr^3 keeps it to ~1e-12 relative (and, as
+            // lambda_min >= 4 det / tr^2 and lambda_max <= tr, far above pinv's cutoff). MAC-VO's 2D->3D covariances are
+            // long thin ellipsoids along the viewing ray (det / tr^3 ~ 1 / condition^2 ~ 1e-15), where the cofactor
+            // inverse is off by 1e-4; those get the Jacobi eigen-decomposition (as accurate as pinv's SVD). An eigenvalue
+            // pinv drops is flagged; a non-finite block keeps zero weight (flagged).
             const double m00 = M[0], m01 = 0.5 * (M[1] + M[3]), m02 = 0.5 * (M[2] + M[6]), m11 = M[4], m12 = 0.5 * (M[5] + M[7]), m22 = M[8];
             const double c00 = m11 * m22 - m12 * m12, c01 = m02 * m12 - m01 * m22, c02 = m01 * m12 - m02 * m11;
-            const double det = m00 * c00 + m01 * c01 + m02 * c02;
-            const double scl = fabs(m00 * m11 * m22) + 1e-300;
-            if (fabs(det) > 1e-13 * scl && isfinite(det)) {
+            const double c22 = m00 * m11 - m01 * m01;
+            const double det = m00 * c00 + m01 * c01 + m02 * c02, tr = m00 + m11 + m22;
+            if (!isfinite(det) || !isfinite(tr)) { w00 = w01 = w02 = w11 = w12 = w22 = 0.0; singular = true; }
+            else if (m00 > 0.0 && c22 > 0.0 && det >= 1e-6 * tr * tr * tr) {      // Sylvester: positive definite
                 const double id = 1.0 / det;
                 w00 = c00 * id; w01 = c01 * id; w02 = c02 * id;
-                w11 = (m00 * m22 - m02 * m02) * id; w12 = (m01 * m02 - m00 * m12) * id; w22 = (m00 * m11 - m01 * m01) * id;
-            } else { w00 = w01 = w02 = w11 = w12 = w22 = 0.0; singular = true; }
+                w11 = (m00 * m22 - m02 * m02) * id; w12 = (m01 * m02 - m00 * m12) * id; w22 = c22 * id;
+            } else singular = sym3_pinv(m00, m01, m02, m11, m12, m22, w00, w01, w02, w11, w12, w22);
         } else {
             double pc[3];
             to_camera(T, P.pos + 3 * k, pc);
@@ -226,19 +286,34 @@ __device__ void accumulate_full(const Problem& P, const double* posevec, Shared&
             j2v = hd * jp0;
             // information matrix of the block: inverse of [[a, c, 0], [c, b, 0], [0, 0, e]]
             const double ca = P.uvcov[3 * k], cb = P.uvcov[3 * k + 1], cc = P.uvcov[3 * k + 2], ce = P.gtype == 0 ? P.dcov[k] : 1.0;
-            // the reference takes torch.pinverse of every covariance block (Optimizer.py:96-99): identical to the inverse
-            // for the positive-definite blocks of this path; a rank-deficient block gets its Moore-Penrose weight (rank-1
-            // symmetric M: M / trace(M)^2; zero block: zero weight) instead of inf / NaN, and is reported in stats[7]
-            const double det = ca * cb - cc * cc, scale2 = ca * cb + cc * cc;
-            if (fabs(det) > 1e-14 * scale2 && isfinite(det)) {
+            // the reference takes torch.pinverse of every covariance block (Optimizer.py:96-99): the inverse when every
+            // eigenvalue of the block ("disp": the 3x3 diag(pixel 2x2, e); "reproj": the 2x2) exceeds PINV_RCOND times the
+            // largest one; otherwise the dropped directions get zero weight (rank-1 pixel block M: M / trace(M)^2) instead
+            // of a huge or inf / NaN one, and the block is reported in stats[7]
+            // |det| / lbig is the smallest |eigenvalue| of the pixel block, lbig its largest; the row-sum bound
+            // lbig <= |a| + |b| + |c| settles the common well-conditioned block without a square root or a division
+            const double det = ca * cb - cc * cc, bnd = fabs(ca) + fabs(cb) + fabs(cc);
+            const double e_abs = P.gtype == 0 && isfinite(ce) ? fabs(ce) : 0.0;
+            double lbig = -1.0;
+            auto largest = [&]() {
+                if (lbig < 0.0) { const double hd2 = 0.5 * (ca - cb); lbig = fabs(0.5 * (ca + cb)) + sqrt(hd2 * hd2 + cc * cc); }
+                return lbig;
+            };
+            const bool full = fabs(det) > PINV_RCOND * fmax(bnd, e_abs) * bnd ||
+                              (largest() > 0.0 && fabs(det) / largest() > PINV_RCOND * fmax(largest(), e_abs));
+            if (!isfinite(det) || !isfinite(bnd)) { w00 = w11 = w01 = 0.0; singular = true; }
+            else if (full) {
                 const double idet = 1.0 / det;
                 w00 = cb * idet; w11 = ca * idet; w01 = -cc * idet;
             } else {
-                const double tr = ca + cb, itr2 = (tr * tr > 0.0 && isfinite(tr)) ? 1.0 / (tr * tr) : 0.0;
+                const double tr = ca + cb, itr2 = largest() > PINV_RCOND * e_abs ? 1.0 / (tr * tr) : 0.0;
                 w00 = ca * itr2; w11 = cb * itr2; w01 = cc * itr2;
                 singular = true;
             }
-            if (fabs(ce) > 0.0 && isfinite(ce)) w22 = 1.0 / ce; else { w22 = 0.0; singular = true; }
+            if (P.gtype == 1) w22 = 1.0;                                             // reproj: no third residual
+            else if (isfinite(ce) && ce != 0.0 &&                                    // a non-finite pixel block leaves e alone
+                     (!isfinite(bnd) || e_abs > PINV_RCOND * bnd || e_abs > PINV_RCOND * largest())) w22 = 1.0 / ce;
+            else { w22 = 0.0; singular = true; }
         }
         const double nrm2 = r[0] * r[0] + r[1] * r[1] + r[2] * r[2];
         const double sn = sqrt(nrm2);
@@ -556,10 +631,17 @@ pgo_accumulate_kernel(Problem P, const double* __restrict__ pose, double* __rest
     __shared__ Shared S;
     cg::cluster_group cluster = cg::this_cluster();
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int rank = (int)cluster.block_rank();
     if (threadIdx.x < 7) S.pose[threadIdx.x] = pose[threadIdx.x];
     __syncthreads();
-    accumulate_full(P, S.pose, S, cluster, warp, WARPS, warp, lane);
-    if (threadIdx.x < NACC) acc_out[threadIdx.x] = S.total[threadIdx.x];
+    accumulate_full(P, S.pose, S, cluster, rank * WARPS + warp, (int)cluster.num_blocks() * WARPS, warp, lane);
+    if (rank == 0 && threadIdx.x < NACC) acc_out[threadIdx.x] = S.total[threadIdx.x];
+}
+
+// CTAs per cluster: the given 1..8, or (0) chosen from the block count
+int cluster_size(int cluster, int k) {
+    if (cluster <= 0) cluster = k >= 2048 ? 8 : (k >= 768 ? 4 : (k >= 256 ? 2 : 1));
+    return cluster > 8 ? 8 : cluster;
 }
 
 int launch_cluster(const void* fn, int cluster, void** args, cudaStream_t st) {
@@ -595,9 +677,7 @@ static int pgo_solve_impl(const double* pos_Tw, const double* kp2_uv, const doub
     if (k > 0 && gx.gtype == 2 && (!gx.pc_obs || !gx.obs_cov || !gx.pts_cov)) return MACVO_E_ARG;
     macvo_pgo_params_t prm = *params;
     if (prm.max_steps < 1 || prm.radius <= 0 || prm.huber_delta <= 0) return MACVO_E_ARG;
-    int cluster = prm.cluster;
-    if (cluster <= 0) cluster = k >= 2048 ? 8 : (k >= 768 ? 4 : (k >= 256 ? 2 : 1));
-    if (cluster > 8) cluster = 8;
+    const int cluster = cluster_size(prm.cluster, k);
     Problem P;
     P.pos = pos_Tw; P.uv = kp2_uv; P.disp = kp2_disp; P.uvcov = uv_cov; P.dcov = disp_cov; P.k = k;
     P.k_dev = k_dev; P.k_offset = k_offset; P.min_k = min_k; P.singular_flag = stats ? stats + 7 : nullptr;
@@ -690,17 +770,30 @@ extern "C" int macvo_pgo_solve_sharded(const double* pos_Tw, const double* kp2_u
                           stream, exchange_bufs, world, rank, k_offset);
 }
 
-extern "C" int macvo_pgo_accumulate(const double* pos_Tw, const double* kp2_uv, const double* kp2_disp,
-                                    const double* uv_cov, const double* disp_cov, int k, const double* intr,
-                                    const double* pose, double huber_delta, double* acc, void* stream) {
-    if (k < 0 || !intr || !pose || !acc) return MACVO_E_ARG;
-    if (k > 0 && (!pos_Tw || !kp2_uv || !kp2_disp || !uv_cov || !disp_cov)) return MACVO_E_ARG;
+extern "C" int macvo_pgo_accumulate_graph(int graph_type, const double* pos_Tw, const double* kp2_uv, const double* kp2_disp,
+                                          const double* uv_cov, const double* disp_cov, const double* pc_obs,
+                                          const double* obs_cov, const double* pts_cov, int k, const double* intr,
+                                          const double* pose, double huber_delta, int cluster, double* acc,
+                                          double* singular_flag, void* stream) {
+    if (k < 0 || !intr || !pose || !acc || graph_type < 0 || graph_type > 2 || cluster < 0 || cluster > 8) return MACVO_E_ARG;
+    if (k > 0 && !pos_Tw) return MACVO_E_ARG;
+    if (k > 0 && graph_type == 0 && (!kp2_uv || !kp2_disp || !uv_cov || !disp_cov)) return MACVO_E_ARG;
+    if (k > 0 && graph_type == 1 && (!kp2_uv || !uv_cov)) return MACVO_E_ARG;
+    if (k > 0 && graph_type == 2 && (!pc_obs || !obs_cov || !pts_cov)) return MACVO_E_ARG;
     Problem P;
     P.pos = pos_Tw; P.uv = kp2_uv; P.disp = kp2_disp; P.uvcov = uv_cov; P.dcov = disp_cov; P.k = k;
-    P.k_dev = nullptr; P.k_offset = 0; P.min_k = 0; P.singular_flag = nullptr; P.world = 1; P.rank = 0;
-    P.gtype = 0; P.pc_obs = P.obs_cov = P.pts_cov = nullptr;
+    P.k_dev = nullptr; P.k_offset = 0; P.min_k = 0; P.singular_flag = singular_flag; P.world = 1; P.rank = 0;
+    P.gtype = graph_type; P.pc_obs = pc_obs; P.obs_cov = obs_cov; P.pts_cov = pts_cov;
     P.K.fx = intr[0]; P.K.fy = intr[1]; P.K.cx = intr[2]; P.K.cy = intr[3]; P.K.bl = intr[4];
     P.delta = huber_delta;
     void* args[] = {&P, &pose, &acc};
-    return launch_cluster(reinterpret_cast<const void*>(&pgo_accumulate_kernel), 1, args, as_stream(stream));
+    return launch_cluster(reinterpret_cast<const void*>(&pgo_accumulate_kernel), cluster_size(cluster, k), args,
+                          as_stream(stream));
+}
+
+extern "C" int macvo_pgo_accumulate(const double* pos_Tw, const double* kp2_uv, const double* kp2_disp,
+                                    const double* uv_cov, const double* disp_cov, int k, const double* intr,
+                                    const double* pose, double huber_delta, double* acc, void* stream) {
+    return macvo_pgo_accumulate_graph(MACVO_PGO_DISP, pos_Tw, kp2_uv, kp2_disp, uv_cov, disp_cov, nullptr, nullptr, nullptr, k,
+                                      intr, pose, huber_delta, 1, acc, nullptr, stream);
 }

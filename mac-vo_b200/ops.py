@@ -97,6 +97,8 @@ EXPORTS = {
                                 + [C.POINTER(_PgoParams)] + [C.c_void_p] * 2 + [C.c_int, C.c_int, C.c_void_p]),
     "macvo_pgo_accumulate": (C.c_int, [C.c_void_p] * 5 + [C.c_int] + [C.c_void_p] * 2 + [C.c_double]
                              + [C.c_void_p] * 2),
+    "macvo_pgo_accumulate_graph": (C.c_int, [C.c_int] + [C.c_void_p] * 8 + [C.c_int] + [C.c_void_p] * 2
+                                   + [C.c_double, C.c_int] + [C.c_void_p] * 3),
     "macvo_layer_norm": (C.c_int, [C.c_void_p] * 4 + [C.c_longlong, C.c_int, C.c_float, C.c_void_p]),
     "macvo_add_layer_norm": (C.c_int, [C.c_void_p] * 6 + [C.c_longlong, C.c_int, C.c_float, C.c_void_p]),
     "macvo_mlp_tc": (C.c_int, [C.c_void_p] * 7 + [C.c_int] * 3 + [C.c_void_p]),
@@ -609,12 +611,34 @@ def pgo_solve_graph(graph_type: str, pos_Tw: Tensor, intr: tuple[float, float, f
     return solve[1], solve[3]
 
 
-def pgo_accumulate(pos_Tw: Tensor, kp2_uv: Tensor, kp2_disp: Tensor, uv_cov: Tensor, disp_cov: Tensor,
-                   intr: tuple[float, float, float, float, float], pose: Tensor, huber_delta: float = 0.1) -> Tensor:
-    P = [_arg(t, F64, f"pgo_accumulate arg{i}", copy=True) for i, t in enumerate((pos_Tw, kp2_uv, kp2_disp, uv_cov, disp_cov))]
+_PGO_COLUMNS = {"disp": ("kp2_uv", "kp2_disp", "uv_cov", "disp_cov"), "reproj": ("kp2_uv", "uv_cov"),
+                "icp": ("pc_obs", "obs_cov", "pts_cov")}
+
+
+def pgo_accumulate(pos_Tw: Tensor, kp2_uv: Tensor | None, kp2_disp: Tensor | None, uv_cov: Tensor | None,
+                   disp_cov: Tensor | None, intr: tuple[float, float, float, float, float], pose: Tensor,
+                   huber_delta: float = 0.1, graph_type: str = "disp", pc_obs: Tensor | None = None,
+                   obs_cov: Tensor | None = None, pts_cov: Tensor | None = None, cluster: int = 1,
+                   singular_flag: Tensor | None = None) -> Tensor:
+    """The 55-double packed normal equations at `pose` (include/macvo_b200.h, macvo_pgo_accumulate_graph) for any graph
+    type; CUDA float64 inputs, the columns a graph type does not read may be None. `cluster`: CTAs reducing the blocks
+    (1..8, 0 = chosen from the block count). `singular_flag` (one float64) is set to 1 when a block lost an eigenvalue to
+    the pseudo-inverse weight."""
+    gt = PGO_GRAPH_TYPES[graph_type]
+    cols = dict(kp2_uv=kp2_uv, kp2_disp=kp2_disp, uv_cov=uv_cov, disp_cov=disp_cov, pc_obs=pc_obs, obs_cov=obs_cov,
+                pts_cov=pts_cov)
+    missing = [n for n in _PGO_COLUMNS[graph_type] if cols[n] is None]
+    if missing:
+        raise MacvoB200Error(f"pgo_accumulate: graph type {graph_type!r} needs {', '.join(missing)}")
+    if not 0 <= int(cluster) <= 8:
+        raise MacvoB200Error(f"pgo_accumulate: cluster must be 0..8, got {cluster}")
+    pos = _arg(pos_Tw, F64, "pgo_accumulate pos_Tw", copy=True)
+    arrs = [_arg(t, F64, f"pgo_accumulate {n}", copy=True, optional=True) for n, t in cols.items()]
     ps = _arg(pose, F64, "pgo_accumulate pose", copy=True).reshape(7)
+    flag = _arg(singular_flag, F64, "pgo_accumulate singular_flag", numel=1, optional=True)
     acc = torch.empty((PGO_ACC,), dtype=torch.float64, device=ps.device)
-    _launch("macvo_pgo_accumulate", *P, P[0].shape[0], _intr(intr), ps, float(huber_delta), acc)
+    _launch("macvo_pgo_accumulate_graph", gt, pos, *arrs, pos.shape[0], _intr(intr), ps, float(huber_delta), int(cluster),
+            acc, flag)
     return acc
 
 

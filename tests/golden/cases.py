@@ -298,6 +298,67 @@ def pgo_inputs_typed(graph_type: str, K: int, seed: int) -> dict:
     return c
 
 
+# focal length -> image size (W, H) of the MAC-VO-shaped icp inputs: TartanAir 640x480, KITTI 1241x376, a 1280x720 camera
+PGO_MACVO_CAMERAS = {320.0: (640, 480), 718.0: (1241, 376), 1000.0: (1280, 720)}
+
+
+def project2to3_cov(u, v, d, depth_var, var_u, var_v, var_uv, fx, fy, cx, cy) -> np.ndarray:
+    """(K,3,3) float64 camera-frame (NED) covariance of a back-projected pixel: the Project2to3 formula of
+    oracle.covariance.match_covariance, evaluated in float64"""
+    s_xx = ((u - cx) ** 2 * depth_var + d ** 2 * var_u + var_u * depth_var) / fx ** 2
+    s_yy = ((v - cy) ** 2 * depth_var + d ** 2 * var_v + var_v * depth_var) / fy ** 2
+    s_xy = ((u - cx) * (v - cy) * depth_var + (d ** 2 + depth_var) * var_uv) / (fx * fy)
+    s_xz, s_yz = depth_var * (u - cx) / fx, depth_var * (v - cy) / fy
+    rows = [[depth_var, s_xz, s_yz], [s_xz, s_xx, s_xy], [s_yz, s_xy, s_yy]]
+    return np.stack([np.stack(r, -1) for r in rows], -2)
+
+
+def pgo_inputs_macvo(K: int, seed: int, fx: float) -> dict:
+    """icp inputs whose covariances look like MAC-VO's: obs_cov / pts_cov are the Project2to3 covariances of the same point
+    seen in frame 2 and in frame 1 (= world), long thin ellipsoids along the viewing ray. Pixels cover the image and a
+    quarter sit within 1.5 % of a corner; depth 1 - 80 m and depth variance 0.05 - 1e5 log-uniform; flow variance at the
+    0.0625 clamp for half the pixels, up to 25 for the rest, a quarter correlated in u / v. Layout as `pgo_inputs_typed`."""
+    from oracle import pgo as opgo
+    rng = np.random.default_rng(seed * 15485863 + K + int(fx))
+    W, H = PGO_MACVO_CAMERAS[fx]
+    fy, cx, cy = fx, W / 2.0, H / 2.0
+    true_pose = opgo.se3_exp(np.array([0.15, -0.05, 0.05, 0.02, -0.03, 0.02]))
+    u, v = rng.uniform(0, W - 1, K), rng.uniform(0, H - 1, K)
+    corner = rng.uniform(size=K) < 0.25
+    n = int(corner.sum())
+    u[corner] = np.where(rng.uniform(size=n) < 0.5, 0.0, W - 1) + rng.uniform(-0.015, 0.015, n) * W
+    v[corner] = np.where(rng.uniform(size=n) < 0.5, 0.0, H - 1) + rng.uniform(-0.015, 0.015, n) * H
+    u, v = np.clip(u, 0, W - 1), np.clip(v, 0, H - 1)
+    d2 = np.exp(rng.uniform(np.log(1.0), np.log(80.0), K))
+    pc2 = np.stack([d2, (u - cx) / fx * d2, (v - cy) / fy * d2], -1)            # frame-2 camera, NED (x forward)
+    pw = opgo.se3_act(true_pose, pc2)                                            # frame 1 = world
+    u1, v1 = fx * pw[:, 1] / pw[:, 0] + cx, fy * pw[:, 2] / pw[:, 0] + cy
+
+    def flow_var():
+        vu, vv = np.full(K, 0.0625), np.full(K, 0.0625)
+        above = rng.uniform(size=K) < 0.5
+        vu[above] = np.exp(rng.uniform(np.log(0.0625), np.log(25.0), int(above.sum())))
+        vv[above] = np.exp(rng.uniform(np.log(0.0625), np.log(25.0), int(above.sum())))
+        rho = np.where(rng.uniform(size=K) < 0.25, rng.uniform(-0.5, 0.5, K), 0.0)
+        return vu, vv, rho * np.sqrt(vu * vv)
+
+    depth_var = lambda: np.exp(rng.uniform(np.log(0.05), np.log(1e5), K))
+    obs_cov = project2to3_cov(u, v, d2, depth_var(), *flow_var(), fx, fy, cx, cy)
+    pts_cov = project2to3_cov(u1, v1, pw[:, 0], depth_var(), *flow_var(), fx, fy, cx, cy)
+    # observations: 1 % depth noise, 0.3 px pixel noise, 5 % gross outliers
+    kp2_uv = np.stack([u, v], -1) + rng.normal(size=(K, 2)) * 0.3
+    kp2_d = d2 * (1 + rng.normal(size=K) * 0.01)
+    out = rng.uniform(size=K) < 0.05
+    kp2_uv[out] += rng.uniform(5, 30, (int(out.sum()), 2))
+    f32 = lambda a: torch.tensor(np.asarray(a), dtype=torch.float32)
+    return {
+        "pos_Tw": f32(pw), "kp2_uv": f32(kp2_uv), "kp2_disp": f32(fx * 0.25 / kp2_d), "uv_cov": f32(np.tile([0.0625, 0.0625, 0.0], (K, 1))),
+        "disp_cov": f32(np.full(K, 0.1)), "K": torch.tensor([[fx, 0., cx], [0., fy, cy], [0., 0., 1.]]), "baseline": 0.25,
+        "init_pose": torch.tensor([0., 0., 0., 0., 0., 0., 1.]), "true_pose": torch.tensor(true_pose),
+        "kp2_d": f32(kp2_d), "obs_cov": torch.tensor(obs_cov), "pts_cov": torch.tensor(pts_cov), "graph_type": "icp",
+    }
+
+
 def pgo_graph(c: dict):
     """cases dict -> oracle.pgo.GraphData (fp32 values promoted to fp64, like `.to(torch.double)`)."""
     from oracle import pgo as opgo

@@ -162,6 +162,22 @@ def test_layer_ops_refuse_cpu_tensors(lib):
         assert ops.LAUNCHES[0] == n0, name
 
 
+def test_pgo_accumulate_refuses_cpu_tensors_for_every_graph_type(lib):
+    """pgo_accumulate's other graph types (graph_type=, the icp columns) refuse CPU operands too, and a graph type's
+    missing column before any operand is looked at"""
+    import torch
+    from macvo_b200 import ops
+    f64 = lambda *s: torch.zeros(*s, dtype=torch.float64)
+    pos, uv, uvc, intr = f64(5, 3), f64(5, 2), f64(5, 3), (1.0,) * 5
+    icp = dict(pc_obs=f64(5, 3), obs_cov=f64(5, 3, 3), pts_cov=f64(5, 3, 3))
+    for call in (lambda: ops.pgo_accumulate(pos, uv, None, uvc, None, intr, f64(7), graph_type="reproj", cluster=2),
+                 lambda: ops.pgo_accumulate(pos, None, None, None, None, intr, f64(7), graph_type="icp", cluster=8, **icp)):
+        with pytest.raises(ops.MacvoB200Error, match="expected a CUDA tensor"):
+            call()
+    with pytest.raises(ops.MacvoB200Error, match="needs pts_cov"):
+        ops.pgo_accumulate(pos, None, None, None, None, intr, f64(7), graph_type="icp", **dict(icp, pts_cov=None))
+
+
 def test_every_public_wrapper_is_checked():
     """a new public function of ops is either host-only or gets a CPU-tensor case above (and a device case in
     tests/test_gpu_ops_args.py)"""

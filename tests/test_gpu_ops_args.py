@@ -186,6 +186,31 @@ def test_pgo_solve_sharded_checks_pose_stats_and_count(ops, which):
         _refused(ops, lambda: ops.pgo_solve_sharded(shard, (1.0,) * 5, None, exchange, **dict(good, **{which: bad})))
 
 
+def test_pgo_accumulate_checks_graph_columns_cluster_and_flag(ops):
+    """every graph type launches with its own columns; a missing column, a cluster size outside 0..8 or a bad flag buffer
+    is refused before the launch"""
+    pos, uv, disp, uvc, dc = f64(5, 3), f64(5, 2), f64(5), f64(5, 3), f64(5)
+    icp = dict(pc_obs=f64(5, 3), obs_cov=f64(5, 3, 3), pts_cov=f64(5, 3, 3))
+    intr = (1.0,) * 5
+    calls = {"disp": lambda **kw: ops.pgo_accumulate(pos, uv, disp, uvc, dc, intr, f64(7), **kw),
+             "reproj": lambda **kw: ops.pgo_accumulate(pos, uv, None, uvc, None, intr, f64(7), graph_type="reproj", **kw),
+             "icp": lambda **kw: ops.pgo_accumulate(pos, None, None, None, None, intr, f64(7), graph_type="icp",
+                                                    **dict(icp, **kw))}
+    for gt, call in calls.items():
+        del ops.stub.calls[:]
+        call(cluster=0, singular_flag=f64(1))
+        call(cluster=8)
+        assert ops.stub.calls == ["macvo_pgo_accumulate_graph"] * 2, gt
+        for bad in (dict(cluster=-1), dict(cluster=9), dict(singular_flag=f64(2)), dict(singular_flag=z(1)),
+                    dict(singular_flag=f64(1).cpu())):
+            _refused(ops, lambda: call(**bad))
+    _refused(ops, lambda: ops.pgo_accumulate(pos, None, disp, uvc, dc, intr, f64(7)))
+    _refused(ops, lambda: ops.pgo_accumulate(pos, uv, None, None, None, intr, f64(7), graph_type="reproj"))
+    _refused(ops, lambda: ops.pgo_accumulate(pos, None, None, None, None, intr, f64(7), graph_type="icp",
+                                             **dict(icp, pts_cov=None)))
+    _refused(ops, lambda: calls["icp"](obs_cov=f64(5, 3, 3).cpu()))
+
+
 @pytest.mark.parametrize("which", ["rows", "mf32", "mf16_rows"])
 def test_flow_im2col_checks_its_outputs(ops, which):
     good = dict(rows=z(4, 128, dtype=torch.float16), mf32=z(4, 128),
